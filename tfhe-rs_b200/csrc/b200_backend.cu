@@ -560,7 +560,7 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
       launch_reg(pbs_n2048_k1_l1_v6_kernel<2, true, 1>, sizeof(P22SmemV6<2, true>),
                  "n2048_v6<2,true,1>");
     } else if (variant == 20) {
-      // v6 hybrid without the CTA barrier after the MAC (split arrive / wait)
+      // the shipped two-CTA instance (lane-pair layout, see below)
       launch_reg(pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1>, sizeof(P22SmemV6<2, true>),
                  "n2048_v6<2,true,2,1>");
     } else if (variant == 22) {
@@ -589,10 +589,13 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
     } else {
       // shipped, two CTAs per SM: v6 hybrid -- own key row prefetched into
       // registers, other row (the one v3 waited a full L2 round trip for)
-      // through the ring, exchange 2 through warp shuffles; rotate + decompose
-      // with the sign as a predicate (CVT = 2); no CTA barrier after the MAC
-      // (SPLIT_POST = 1: the two groups of a CTA only exchange arrive / wait
-      // signals there)
+      // through the ring; rotate + decompose with the sign as a predicate
+      // (CVT = 2); lane-pair layout: each warp holds the same 16 threads of
+      // both polynomials (lanes l and l ^ 16), exchange 2 through half-warp
+      // shuffles, the other polynomial's spectrum taken with one shuffle in
+      // the MAC (no spectrum store, no barrier between the polynomials).
+      // Bit-identical to variant 17, the same instance in the 64-thread
+      // group layout.
       launch_reg(pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1>, sizeof(P22SmemV6<2, true>),
                  "n2048_v6<2,true,2,1>");
     }

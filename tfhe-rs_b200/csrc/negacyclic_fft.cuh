@@ -330,6 +330,47 @@ B200_HD void x1t_store_p2(cplx *buf, int t, const cplx v[16]) {
     for (int a = 0; a < 4; a++)
       buf[x1t_slot(q, 16 * a + 4 * bh + bl)] = v[4 * bl + a];
 }
+// ---------------------------------------------------------------------------
+// Exchange 1 for the lane-pair layout (half-warp exchange 2, x2h_* in
+// x2_shfl.cuh): warp w holds t = 16 w + i (i = lane & 15) of BOTH polynomials,
+// polynomial 0 on lanes 0-15 and polynomial 1 on lanes 16-31, each in its own
+// buffer.  Pass-2 work: half-lane p + 4 m <-> (sub-problem q = 4 w + p,
+// quarter bh = m).  A pass-2 quarter-warp holds 4 q (p = 0..3) and 2 quarters,
+// so the j0 it reads differ in bit 2 (bh) and in bits 0-1 only through the
+// swizzle by q & 3:  X1H slot of element (q, j0) = q*64 + (j0 ^ (q & 3)).  A
+// pass-1 quarter-warp holds 8 aligned consecutive j0 and one q.  Both sides hit
+// 8 distinct 16-byte bank groups (emu_lanepair_conflict_audit).
+// Warp w's pass-2 accesses stay in rows 4 w .. 4 w + 3 of each buffer.
+// ---------------------------------------------------------------------------
+B200_HD int x1h_slot(int q, int j0) { return q * 64 + (j0 ^ (q & 3)); }
+B200_HD int x1h_q(int t) { return ((t >> 4) << 2) | (t & 3); }
+B200_HD int x1h_bh(int t) { return (t >> 2) & 3; }
+B200_HD void x1h_store_p1(cplx *buf, int t, const cplx v[16]) {
+#pragma unroll
+  for (int q = 0; q < 16; q++)
+    buf[x1h_slot(q, t)] = v[q];
+}
+B200_HD void x1h_load_p1(const cplx *buf, int t, cplx v[16]) {
+#pragma unroll
+  for (int q = 0; q < 16; q++)
+    v[q] = buf[x1h_slot(q, t)];
+}
+B200_HD void x1h_load_p2(const cplx *buf, int t, cplx v[16]) {
+  const int q = x1h_q(t), bh = x1h_bh(t);
+#pragma unroll
+  for (int bl = 0; bl < 4; bl++)
+#pragma unroll
+    for (int a = 0; a < 4; a++)
+      v[4 * bl + a] = buf[x1h_slot(q, 16 * a + 4 * bh + bl)];
+}
+B200_HD void x1h_store_p2(cplx *buf, int t, const cplx v[16]) {
+  const int q = x1h_q(t), bh = x1h_bh(t);
+#pragma unroll
+  for (int bl = 0; bl < 4; bl++)
+#pragma unroll
+    for (int a = 0; a < 4; a++)
+      buf[x1h_slot(q, 16 * a + 4 * bh + bl)] = v[4 * bl + a];
+}
 // spectrum layout used for sharing and for the Fourier BSK: index b*64 + t
 B200_HD void spec_store(cplx *buf, int t, const cplx v[16]) {
 #pragma unroll

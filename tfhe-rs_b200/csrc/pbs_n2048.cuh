@@ -569,11 +569,15 @@ pbs_n2048_k1_l1_v3_kernel(uint64_t *__restrict__ lwe_out,
 // staged in shared memory (2 KiB) -- otherwise step i recomputes a_hat[i] from
 // the input LWE word, loaded one step ahead: with the 64 KiB ring the 2 KiB
 // would push the CTA over half an SM's shared memory.
+// The rows of acc are 16 words apart modulo the 32 banks: in the lane-pair
+// layout a warp reads and writes the same 16 coefficients of both polynomials,
+// and the two halves then hit disjoint banks.
+constexpr int P22_ACC_STRIDE = P22_N + 16;
 template <int RING, bool STAGE_A>
 struct P22SmemV6 {
   cplx xa[2][P22_M];        // 32 KiB  exchange 1 / spectrum share
   cplx ring[RING][P22_M];   // key blocks of one step
-  uint32_t acc[2][P22_N];   // 16 KiB
+  uint32_t acc[2][P22_ACC_STRIDE]; // 16 KiB + 128 B
   uint16_t a_hat[STAGE_A ? 1024 + 8 : 4];
   uint32_t b_hat;
   unsigned long long red_half[4];
@@ -609,11 +613,13 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
                           uint32_t lut_stride, int centered_ms) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   constexpr int RING = KEY_MODE == 0 ? 4 : KEY_MODE == 2 ? 2 : 1;
+  // The shipped two-CTA instance runs the lane-pair layout (see the loop).
+  constexpr bool LANE_PAIR = KEY_MODE == 2 && STAGE_A && CVT == 2 && SPLIT_POST == 1;
   using Smem = P22SmemV6<RING, STAGE_A>;
   Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
   const int tid = threadIdx.x;
-  const int g = tid >> 6;
-  const int t = tid & 63;
+  const int g = LANE_PAIR ? (tid >> 4) & 1 : tid >> 6;
+  const int t = LANE_PAIR ? ((tid >> 5) << 4) | (tid & 15) : tid & 63;
   const uint32_t s = blockIdx.x;
   const uint32_t log_mod = 12;
 
@@ -705,7 +711,7 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
   cplx tw2[3], tw3[15];
 #pragma unroll
   for (int e = 0; e < 3; e++)
-    tw2[e] = tables->pass2[x1t_q(t)][e];
+    tw2[e] = tables->pass2[LANE_PAIR ? x1h_q(t) : x1t_q(t)][e];
 #pragma unroll
   for (int e = 0; e < 15; e++)
     tw3[e] = tables->pass3[t][e];
@@ -713,118 +719,168 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
 
   uint32_t *acc_g = sm.acc[g];
   cplx *xa_g = sm.xa[g];
-  const cplx *xa_other = sm.xa[1 - g];
+  [[maybe_unused]] const cplx *xa_other = sm.xa[1 - g];
   // ring slot of block 2c + r: RING = 4 -> 2c + r; RING = 2 -> blocks 1, 2 at 0, 1
   [[maybe_unused]] const cplx *k_own = &sm.ring[RING == 4 ? 2 * g + g : 0][0];
   const cplx *k_oth = &sm.ring[RING == 4 ? 2 * g + (1 - g) : RING == 2 ? g : 0][0];
   const cplx *bsk_own = bsk + (size_t)g * (2 * P22_M) + (size_t)g * P22_M + t;
-  const cplx *bsk_oth = bsk + (size_t)g * (2 * P22_M) + (size_t)(1 - g) * P22_M;
+  [[maybe_unused]] const cplx *bsk_oth =
+      bsk + (size_t)g * (2 * P22_M) + (size_t)(1 - g) * P22_M;
   uint32_t own[32];
   p22v4_own_init(acc_g, t, own);
   [[maybe_unused]] uint64_t ct_next = (!STAGE_A && n > 0) ? ct[0] : 0;
   [[maybe_unused]] uint32_t a_next = (STAGE_A && n > 0) ? sm.a_hat[0] : 0;
-  for (uint32_t i = 0; i < n; i++) {
-    uint32_t a;
-    if constexpr (STAGE_A) {
-      a = a_next; // read a step ahead: every address of the step hangs on it
-      a_next = sm.a_hat[i + 1]; // a_hat has 8 words of padding
-    } else {
-      a = modulus_switch_u64(ct_next, log_mod) & (2 * P22_N - 1);
-      if (i + 1 < n)
-        ct_next = ct[i + 1];
-    }
-    if constexpr (KEY_MODE == 1) {
-      if (a == 0)
-        continue;
-    }
-    cplx v[16];
-    p22v4_load_digits<CVT>(acc_g, t, a, base_log, own, v);
-    radix16_fwd(v, c_fft1024_pass1);
-    x1t_store_p1(xa_g, t, v);
-    group_barrier(g);
-    x1t_load_p2(xa_g, t, v);
-    pass2_fwd(v, tw2);
-    spec_guard_arrive(g, t);
-    x2s_fwd(v);
-    radix16_fwd(v, tw3);
-    if constexpr (KEY_MODE == 0) {
-      spec_guard_wait(g, t);
-      spec_store(xa_g, t, v);
+  if constexpr (LANE_PAIR) {
+    // Lane-pair layout: lane l of warp w runs thread t = 16 w + (l & 15) of
+    // polynomial l >> 4, so lanes l and l ^ 16 hold the same spectrum slots
+    // 16 t + b of the two polynomials after the forward transform.  The MAC
+    // takes the other polynomial's value with one shuffle: no spectrum store,
+    // no barrier between the polynomials before or after it.  Exchange 2 stays
+    // inside each half-warp (x2h_*), exchange 1 goes through xa[g] (x1h_*), and
+    // the values and the order of every operation are those of the other
+    // instances, so the results are bit-identical.
+    for (uint32_t i = 0; i < n; i++) {
+      const uint32_t a = a_next; // read a step ahead: every address of the step hangs on it
+      a_next = sm.a_hat[i + 1];  // a_hat has 8 words of padding
+      cplx v[16];
+      p22v4_load_digits<CVT>(acc_g, t, a, base_log, own, v);
+      radix16_fwd(v, c_fft1024_pass1);
+      x1h_store_p1(xa_g, t, v);
       __syncthreads();
-      mbar_wait_parity(&sm.bar, i & 1u);
-#pragma unroll
-      for (int b = 0; b < 16; b++)
-        v[b] = cfma(xa_other[b * 64 + t], k_oth[b * 64 + t],
-                    cmul(v[b], k_own[b * 64 + t]));
-      if constexpr (SPLIT_POST) {
-        mac_done_arrive(g);
-      } else {
-        __syncthreads();
-        if (tid == 0 && i + 1 < n)
-          tma_issue(i + 1); // every reader of the slot is behind the barrier
-      }
-    } else if constexpr (KEY_MODE == 2) {
-      // own row through registers (requested here, consumed after the share
-      // barrier), other row from the ring: half the ring traffic of mode 0
+      x1h_load_p2(xa_g, t, v);
+      pass2_fwd(v, tw2);
+      x2h_fwd(v);
+      radix16_fwd(v, tw3);
       const size_t step = (size_t)i * (4 * P22_M);
       cplx b_own[16];
 #pragma unroll
       for (int b = 0; b < 16; b++)
         b_own[b] = ldcg_cplx(bsk_own + step + b * 64);
-      spec_guard_wait(g, t);
-      spec_store(xa_g, t, v);
-      if constexpr (SPLIT_POST == 2) {
-        spec_ready_arrive(g);
+      mbar_wait_parity(&sm.bar, i & 1u);
 #pragma unroll
-        for (int b = 0; b < 16; b++)
-          v[b] = cmul(v[b], b_own[b]); // same operation order as below
-        spec_ready_wait(g);
+      for (int b = 0; b < 16; b++) {
+        const cplx o = shfl_xor_cplx(v[b], 16);
+        v[b] = cfma(o, k_oth[b * 64 + t], cmul(v[b], b_own[b]));
+      }
+      radix16_inv(v, tw3);
+      x2h_inv(v);
+      pass2_inv(v, tw2);
+      // the forward exchange-1 loads of this warp read the same slots (rows
+      // 4 w .. 4 w + 3 of xa[g]); no other warp touches them in between
+      __syncwarp();
+      x1h_store_p2(xa_g, t, v);
+      __syncthreads();
+      if (tid == 0 && i + 1 < n)
+        tma_issue(i + 1); // every warp is past its MAC: the slot is free
+      x1h_load_p1(xa_g, t, v);
+      radix16_inv(v, c_fft1024_pass1);
+      p22v4_acc_update(acc_g, t, v, own);
+      __syncthreads();
+    }
+  } else {
+    for (uint32_t i = 0; i < n; i++) {
+      uint32_t a;
+      if constexpr (STAGE_A) {
+        a = a_next; // read a step ahead: every address of the step hangs on it
+        a_next = sm.a_hat[i + 1]; // a_hat has 8 words of padding
+      } else {
+        a = modulus_switch_u64(ct_next, log_mod) & (2 * P22_N - 1);
+        if (i + 1 < n)
+          ct_next = ct[i + 1];
+      }
+      if constexpr (KEY_MODE == 1) {
+        if (a == 0)
+          continue;
+      }
+      cplx v[16];
+      p22v4_load_digits<CVT>(acc_g, t, a, base_log, own, v);
+      radix16_fwd(v, c_fft1024_pass1);
+      x1t_store_p1(xa_g, t, v);
+      group_barrier(g);
+      x1t_load_p2(xa_g, t, v);
+      pass2_fwd(v, tw2);
+      spec_guard_arrive(g, t);
+      x2s_fwd(v);
+      radix16_fwd(v, tw3);
+      if constexpr (KEY_MODE == 0) {
+        spec_guard_wait(g, t);
+        spec_store(xa_g, t, v);
+        __syncthreads();
         mbar_wait_parity(&sm.bar, i & 1u);
 #pragma unroll
         for (int b = 0; b < 16; b++)
-          v[b] = cfma(xa_other[b * 64 + t], k_oth[b * 64 + t], v[b]);
-      } else {
-      __syncthreads();
-      mbar_wait_parity(&sm.bar, i & 1u);
+          v[b] = cfma(xa_other[b * 64 + t], k_oth[b * 64 + t],
+                      cmul(v[b], k_own[b * 64 + t]));
+        if constexpr (SPLIT_POST) {
+          mac_done_arrive(g);
+        } else {
+          __syncthreads();
+          if (tid == 0 && i + 1 < n)
+            tma_issue(i + 1); // every reader of the slot is behind the barrier
+        }
+      } else if constexpr (KEY_MODE == 2) {
+        // own row through registers (requested here, consumed after the share
+        // barrier), other row from the ring: half the ring traffic of mode 0
+        const size_t step = (size_t)i * (4 * P22_M);
+        cplx b_own[16];
 #pragma unroll
-      for (int b = 0; b < 16; b++)
-        v[b] = cfma(xa_other[b * 64 + t], k_oth[b * 64 + t],
-                    cmul(v[b], b_own[b]));
-      }
-      if constexpr (SPLIT_POST) {
-        mac_done_arrive(g);
-      } else {
+        for (int b = 0; b < 16; b++)
+          b_own[b] = ldcg_cplx(bsk_own + step + b * 64);
+        spec_guard_wait(g, t);
+        spec_store(xa_g, t, v);
+        if constexpr (SPLIT_POST == 2) {
+          spec_ready_arrive(g);
+#pragma unroll
+          for (int b = 0; b < 16; b++)
+            v[b] = cmul(v[b], b_own[b]); // same operation order as below
+          spec_ready_wait(g);
+          mbar_wait_parity(&sm.bar, i & 1u);
+#pragma unroll
+          for (int b = 0; b < 16; b++)
+            v[b] = cfma(xa_other[b * 64 + t], k_oth[b * 64 + t], v[b]);
+        } else {
         __syncthreads();
-        if (tid == 0 && i + 1 < n)
-          tma_issue(i + 1);
-      }
-    } else {
-      const size_t step = (size_t)i * (4 * P22_M);
-      cplx b_own[16];
+        mbar_wait_parity(&sm.bar, i & 1u);
 #pragma unroll
-      for (int b = 0; b < 16; b++)
-        b_own[b] = ldcg_cplx(bsk_own + step + b * 64);
-      spec_guard_wait(g, t);
-      spec_store(xa_g, t, v);
-      __syncthreads();
-      p22v3_mac(v, b_own, xa_other, bsk_oth + step, t, LdcgLoader());
-      __syncthreads();
+        for (int b = 0; b < 16; b++)
+          v[b] = cfma(xa_other[b * 64 + t], k_oth[b * 64 + t],
+                      cmul(v[b], b_own[b]));
+        }
+        if constexpr (SPLIT_POST) {
+          mac_done_arrive(g);
+        } else {
+          __syncthreads();
+          if (tid == 0 && i + 1 < n)
+            tma_issue(i + 1);
+        }
+      } else {
+        const size_t step = (size_t)i * (4 * P22_M);
+        cplx b_own[16];
+#pragma unroll
+        for (int b = 0; b < 16; b++)
+          b_own[b] = ldcg_cplx(bsk_own + step + b * 64);
+        spec_guard_wait(g, t);
+        spec_store(xa_g, t, v);
+        __syncthreads();
+        p22v3_mac(v, b_own, xa_other, bsk_oth + step, t, LdcgLoader());
+        __syncthreads();
+      }
+      radix16_inv(v, tw3);
+      x2s_inv(v);
+      pass2_inv(v, tw2);
+      if constexpr (SPLIT_POST && KEY_MODE != 1)
+        mac_done_wait(g); // the other group has read this group's spectrum
+      x1t_store_p2(xa_g, t, v);
+      group_barrier(g);
+      if constexpr (SPLIT_POST && KEY_MODE != 1) {
+        if (tid == 0 && i + 1 < n)
+          tma_issue(i + 1); // both groups are past their MAC: the slot is free
+      }
+      x1t_load_p1(xa_g, t, v);
+      radix16_inv(v, c_fft1024_pass1);
+      p22v4_acc_update(acc_g, t, v, own);
+      group_barrier(g);
     }
-    radix16_inv(v, tw3);
-    x2s_inv(v);
-    pass2_inv(v, tw2);
-    if constexpr (SPLIT_POST && KEY_MODE != 1)
-      mac_done_wait(g); // the other group has read this group's spectrum
-    x1t_store_p2(xa_g, t, v);
-    group_barrier(g);
-    if constexpr (SPLIT_POST && KEY_MODE != 1) {
-      if (tid == 0 && i + 1 < n)
-        tma_issue(i + 1); // both groups are past their MAC: the slot is free
-    }
-    x1t_load_p1(xa_g, t, v);
-    radix16_inv(v, c_fft1024_pass1);
-    p22v4_acc_update(acc_g, t, v, own);
-    group_barrier(g);
   }
   __syncthreads();
 
