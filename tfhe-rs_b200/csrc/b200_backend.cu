@@ -11,8 +11,11 @@
 #include <atomic>
 #include <cstring>
 #include <mutex>
+#include <optional>
+#include <set>
 #include <string>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
@@ -33,10 +36,61 @@
 namespace b200 {
 
 static std::atomic<uint64_t> g_launches{0};
-void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
+
+// kernel<<<grid, block, smem, stream>>> on device `gpu`, and where the launch is
+// made from (for the message of a failed launch).  An instance launched with
+// dynamic shared memory has its limit raised to `smem_max`, once per (instance,
+// device): the most that instance is ever launched with.  It defaults to `smem`
+// (instances of a fixed size); callers whose size varies pass their bound, so
+// the value never depends on which host thread launched first.
+struct LaunchCfg {
+  dim3 grid, block;
+  size_t smem;
+  cudaStream_t stream;
+  uint32_t gpu;
+  size_t smem_max;
+  const char *file;
+  int line;
+  LaunchCfg(dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+            uint32_t gpu, size_t smem_max = 0,
+            const char *file = __builtin_FILE(), int line = __builtin_LINE())
+      : grid(grid), block(block), smem(smem), stream(stream), gpu(gpu),
+        smem_max(smem_max ? smem_max : smem), file(file), line(line) {}
+};
+
+static void check_launch(cudaError_t code, const LaunchCfg &c) {
+  if (code != cudaSuccess) {
+    std::fprintf(stderr, "Cuda error: %s %s %d\n", cudaGetErrorString(code),
+                 c.file, c.line);
+    std::abort();
+  }
+}
+
+static void raise_smem_limit(const void *kernel, const LaunchCfg &c) {
+  static std::mutex mutex;
+  static std::set<std::pair<const void *, uint32_t>> raised;
+  std::lock_guard<std::mutex> lock(mutex);
+  if (raised.emplace(kernel, c.gpu).second)
+    check_launch(cudaFuncSetAttribute(kernel,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)c.smem_max),
+                 c);
+}
+
+// every kernel launch of the library: enqueue, check, count
+// (b200_kernel_launch_count)
+template <typename... Params, typename... Args>
+static void launch(void (*kernel)(Params...), const LaunchCfg &c,
+                   Args &&...args) {
+  if (c.smem)
+    raise_smem_limit(reinterpret_cast<const void *>(kernel), c);
+  kernel<<<c.grid, c.block, c.smem, c.stream>>>(std::forward<Args>(args)...);
+  check_launch(cudaGetLastError(), c);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+}
 
 // name of the kernel instance the calling thread's last PBS launch ran
-// (b200_last_pbs_kernel): one pointer store per launch, next to count_launch
+// (b200_last_pbs_kernel): one pointer store per launch
 static thread_local const char *t_last_pbs_kernel = "";
 // the same for the keyswitch (b200_last_keyswitch_kernel)
 static thread_local const char *t_last_ks_kernel = "";
@@ -154,10 +208,54 @@ static bool uses_n8192_path(uint32_t n, uint32_t k, uint32_t N, uint32_t l) {
 // kernel (u64 accumulator), 3 the round-1 register kernel, 5 round-1 MAC
 // schedule + lean rotate/decompose (the default), 4 all key values in flight
 // across the share barrier + lean rotate/decompose.  Read once per process.
-// kernel generations b200_set_pbs_variant / B200_PBS_VARIANT can pin (see launch_pbs)
-static bool is_pbs_variant(int v) {
-  return v == 0 || v == 1 || (v >= 3 && v <= 11) || (v >= 14 && v <= 22);
+// The N = 2048 kernel instances by the variant b200_set_pbs_variant /
+// B200_PBS_VARIANT pins (0: the automatic choice of launch_pbs).
+struct N2048Instance {
+  int variant;
+  decltype(&pbs_n2048_k1_l1_kernel) kernel;
+  size_t smem;
+  const char *name;
+};
+static const N2048Instance N2048_INSTANCES[] = {
+    // v1: 64-bit accumulator (A/B measurements and base_log = 31)
+    {1, pbs_n2048_k1_l1_kernel, sizeof(P22Smem), "n2048_v1"},
+    {3, pbs_n2048_k1_l1_v3_kernel<0, 0>, sizeof(P22SmemV3), "n2048_v3<0,0>"}, // round 1
+    {4, pbs_n2048_k1_l1_v3_kernel<1, 1>, sizeof(P22SmemV3), "n2048_v3<1,1>"},
+    {5, pbs_n2048_k1_l1_v3_kernel<0, 1>, sizeof(P22SmemV3), "n2048_v3<0,1>"},
+    {6, pbs_n2048_k1_l1_v3_kernel<2, 1>, sizeof(P22SmemV3), "n2048_v3<2,1>"},
+    // TMA ring for the key block: 208 KiB of shared memory, one CTA per SM
+    {7, pbs_n2048_k1_l1_v3_kernel<3, 1>, sizeof(P22SmemV3Tma), "n2048_v3<3,1>"},
+    // exchange 2 through warp shuffles (x2_shfl.cuh)
+    {8, pbs_n2048_k1_l1_v3_kernel<0, 1, 1>, sizeof(P22SmemV3), "n2048_v3<0,1,1>"},
+    // v6: shuffle exchange 2 + one-slot TMA key ring, 2 CTAs / SM
+    {9, pbs_n2048_k1_l1_v6_kernel<0, false>, sizeof(P22SmemV6<4, false>), "n2048_v6<0,false>"},
+    // v6 with v3's register key prefetch (isolates the ring)
+    {10, pbs_n2048_k1_l1_v6_kernel<1, true>, sizeof(P22SmemV6<1, true>), "n2048_v6<1,true>"},
+    // v6 hybrid: own row in registers, other row through the ring
+    {11, pbs_n2048_k1_l1_v6_kernel<2, true>, sizeof(P22SmemV6<2, true>), "n2048_v6<2,true>"},
+    // v6 with the switched mask staged in shared memory: one CTA per SM
+    {14, pbs_n2048_k1_l1_v6_kernel<0, true>, sizeof(P22SmemV6<4, true>), "n2048_v6<0,true>"},
+    // v6 ring, digits converted through the fp64 ADD pipe instead of I2F
+    {15, pbs_n2048_k1_l1_v6_kernel<0, true, 1>, sizeof(P22SmemV6<4, true>), "n2048_v6<0,true,1>"},
+    {16, pbs_n2048_k1_l1_v6_kernel<2, true, 1>, sizeof(P22SmemV6<2, true>), "n2048_v6<2,true,1>"},
+    {17, pbs_n2048_k1_l1_v6_kernel<2, true, 2>, sizeof(P22SmemV6<2, true>), "n2048_v6<2,true,2>"},
+    {18, pbs_n2048_k1_l1_v6_kernel<2, true, 3>, sizeof(P22SmemV6<2, true>), "n2048_v6<2,true,3>"},
+    // the shipped one-CTA instance (see launch_pbs)
+    {19, pbs_n2048_k1_l1_v6_kernel<0, true, 2>, sizeof(P22SmemV6<4, true>), "n2048_v6<0,true,2>"},
+    // the shipped two-CTA instance (lane-pair layout, see launch_pbs)
+    {20, pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1>, sizeof(P22SmemV6<2, true>), "n2048_v6<2,true,2,1>"},
+    {21, pbs_n2048_k1_l1_v6_kernel<0, true, 2, 1>, sizeof(P22SmemV6<4, true>), "n2048_v6<0,true,2,1>"},
+    // v6 hybrid with both CTA barriers of a step split (own-row products before
+    // the wait for the other group's spectrum)
+    {22, pbs_n2048_k1_l1_v6_kernel<2, true, 2, 2>, sizeof(P22SmemV6<2, true>), "n2048_v6<2,true,2,2>"},
+};
+static const N2048Instance *n2048_instance(int variant) {
+  for (const N2048Instance &r : N2048_INSTANCES)
+    if (r.variant == variant)
+      return &r;
+  return nullptr;
 }
+static bool is_pbs_variant(int v) { return v == 0 || n2048_instance(v); }
 static std::atomic<int> &fast_variant_sel() {
   static std::atomic<int> v([] {
     const char *e = std::getenv("B200_PBS_VARIANT");
@@ -226,6 +324,33 @@ struct PbsScratch : public pbs_buffer_base_abi {
   }
   ~PbsScratch() override { magic = 0; }
 };
+
+// (k, N, l) a scratch object is made for
+struct PbsShape {
+  uint32_t glwe_dim, poly_size, level_count;
+};
+
+// the scratch object behind `buffer`, checked to be a live one of `type`; made
+// for `shape` when one is given, and for at least `samples` samples.  `what`
+// names the caller in the messages.
+static const PbsScratch &pbs_scratch(const int8_t *buffer, PBS_TYPE type,
+                                     const char *what,
+                                     std::optional<PbsShape> shape = {},
+                                     uint64_t samples = 0) {
+  const PbsScratch *s = reinterpret_cast<const PbsScratch *>(buffer);
+  B200_PANIC_IF_FALSE(s && s->magic == SCRATCH_MAGIC && s->type == type,
+                      "Cuda error (%s): invalid scratch buffer", what);
+  B200_PANIC_IF_FALSE(
+      !shape || (s->glwe_dim == shape->glwe_dim &&
+                 s->poly_size == shape->poly_size &&
+                 s->level_count == shape->level_count),
+      "Cuda error (%s): scratch buffer was created for other parameters", what);
+  B200_PANIC_IF_FALSE(samples <= s->max_samples,
+                      "Cuda error (%s): scratch buffer made for %u samples, "
+                      "the call runs %llu", what, s->max_samples,
+                      (unsigned long long)samples);
+  return *s;
+}
 
 // stream-ordered workspace pool shared by the entry points that need scratch
 // memory per call (keyswitch digit matrix, multi-bit bundles): freed blocks stay
@@ -297,64 +422,38 @@ static void launch_multibit_ll(cudaStream_t stream, uint32_t gpu_index,
   cplx *bundle = nullptr;
   B200_CHECK(cudaMallocFromPoolAsync(&bundle, bytes, workspace_pool(gpu_index),
                                      stream));
-  static std::once_flag once[MAX_GPUS];
-  std::call_once(once[gpu_index], [] {
-    B200_CHECK(cudaFuncSetAttribute(
-        pbs_multibit_seq_kernel<1, false>,
-        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MbSeqSmem)));
-    B200_CHECK(cudaFuncSetAttribute(
-        pbs_multibit_seq_kernel<2, false>,
-        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MbSeqSmem)));
-    B200_CHECK(cudaFuncSetAttribute(
-        pbs_multibit_seq_kernel<1, true>,
-        cudaFuncAttributeMaxDynamicSharedMemorySize,
-        (int)sizeof(MbSeqSmemTma)));
-  });
-  auto for_each_instance = [&](auto &&fn) {
-    fn(mb_bundle_kernel<2, 1>, 2u, 1u);
-    fn(mb_bundle_kernel<2, 2>, 2u, 2u);
-    fn(mb_bundle_kernel<3, 1>, 3u, 1u);
-    fn(mb_bundle_kernel<3, 2>, 3u, 2u);
-    fn(mb_bundle_kernel<4, 1>, 4u, 1u);
-    fn(mb_bundle_kernel<4, 2>, 4u, 2u);
-  };
-  for_each_instance([&](auto bun, uint32_t kg, uint32_t kl) {
-    if (kg != grouping || kl != l)
-      return;
-    bun<<<dim3(steps, 2, 4), 256, 0, stream>>>(bundle, bsk, t.gen_root[10],
-                                              t.mono2048, lwe_in, in_idx, n,
-                                              num_samples);
-  });
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  // [grouping - 2][l - 1]
+  static const decltype(&mb_bundle_kernel<2, 1>) bundle_kernels[3][2] = {
+      {mb_bundle_kernel<2, 1>, mb_bundle_kernel<2, 2>},
+      {mb_bundle_kernel<3, 1>, mb_bundle_kernel<3, 2>},
+      {mb_bundle_kernel<4, 1>, mb_bundle_kernel<4, 2>}};
+  launch(bundle_kernels[grouping - 2][l - 1],
+         {dim3(steps, 2, 4), 256, 0, stream, gpu_index}, bundle, bsk,
+         t.gen_root[10], t.mono2048, lwe_in, in_idx, n, num_samples);
   // l = 1: the bundle block of a step comes through the bulk-copy (TMA) ring
   // B200_MULTIBIT_SEQ_TMA=0 selects the register-prefetch variant for A/B runs
   static const bool use_tma = [] {
     const char *e = std::getenv("B200_MULTIBIT_SEQ_TMA");
     return !e || std::atoi(e) != 0;
   }();
-  // [grouping - 2][l - 1][register prefetch, TMA ring]
-  static const char *const ll_names[3][2][2] = {
-      {{"multibit_ll<2,1,regs>", "multibit_ll<2,1,tma>"}, {"multibit_ll<2,2,regs>", ""}},
-      {{"multibit_ll<3,1,regs>", "multibit_ll<3,1,tma>"}, {"multibit_ll<3,2,regs>", ""}},
-      {{"multibit_ll<4,1,regs>", "multibit_ll<4,1,tma>"}, {"multibit_ll<4,2,regs>", ""}}};
-  t_last_pbs_kernel = ll_names[grouping - 2][l - 1][l == 1 && use_tma];
-  if (l == 1 && use_tma) {
-    pbs_multibit_seq_kernel<1, true>
-        <<<num_samples, 128, sizeof(MbSeqSmemTma), stream>>>(
-            lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx, bundle, t.fft1024,
-            n, steps, base_log, num_many_lut, lut_stride,
-            multibit_ties_even().load());
-  } else {
-    auto seq = l == 1 ? pbs_multibit_seq_kernel<1, false>
-                      : pbs_multibit_seq_kernel<2, false>;
-    seq<<<num_samples, 128, sizeof(MbSeqSmem), stream>>>(
-        lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx, bundle, t.fft1024, n,
-        steps, base_log, num_many_lut, lut_stride,
-        multibit_ties_even().load());
-  }
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  // [l = 1, l = 2 with register prefetch; l = 1 with the TMA ring], named per
+  // grouping - 2
+  static const struct {
+    decltype(&pbs_multibit_seq_kernel<1, false>) kernel;
+    size_t smem;
+    const char *names[3];
+  } seq_kernels[3] = {
+      {pbs_multibit_seq_kernel<1, false>, sizeof(MbSeqSmem),
+       {"multibit_ll<2,1,regs>", "multibit_ll<3,1,regs>", "multibit_ll<4,1,regs>"}},
+      {pbs_multibit_seq_kernel<2, false>, sizeof(MbSeqSmem),
+       {"multibit_ll<2,2,regs>", "multibit_ll<3,2,regs>", "multibit_ll<4,2,regs>"}},
+      {pbs_multibit_seq_kernel<1, true>, sizeof(MbSeqSmemTma),
+       {"multibit_ll<2,1,tma>", "multibit_ll<3,1,tma>", "multibit_ll<4,1,tma>"}}};
+  const auto &seq = seq_kernels[l == 1 && use_tma ? 2 : l - 1];
+  launch(seq.kernel, {num_samples, 128, seq.smem, stream, gpu_index}, lwe_out,
+         out_idx, luts, lut_idx, lwe_in, in_idx, bundle, t.fft1024, n, steps,
+         base_log, num_many_lut, lut_stride, multibit_ties_even().load());
+  t_last_pbs_kernel = seq.names[grouping - 2];
   B200_CHECK(cudaFreeAsync(bundle, stream));
 }
 
@@ -372,53 +471,47 @@ static void launch_pbs_generic(cudaStream_t stream, uint32_t gpu_index,
   const uint32_t logM = ilog2_exact(N) - 1;
   const DeviceTables &t = device_tables(gpu_index, logM);
   const size_t smem = generic_smem_bytes(grouping > 1 ? 16 : n, k, N, l);
-  int max_smem = 0;
-  B200_CHECK(cudaDeviceGetAttribute(
-      &max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, (int)gpu_index));
-  // The attribute value must not depend on call arguments in a way that races
-  // between host threads: always raise it to the device maximum.
-  static std::once_flag gen_once[MAX_GPUS];
-  cudaFuncAttributes fattr;
-  B200_CHECK(
-      cudaFuncGetAttributes(&fattr, pbs_generic_kernel<256, false, Torus>));
-  const int max_dyn = max_smem - (int)fattr.sharedSizeBytes;
-  std::call_once(gen_once[gpu_index], [max_dyn] {
-    B200_CHECK(cudaFuncSetAttribute(
-        pbs_generic_kernel<256, false, Torus>,
-        cudaFuncAttributeMaxDynamicSharedMemorySize, max_dyn));
+  // The limit is the device maximum, whatever the call: a value taken from
+  // call arguments would race between host threads.
+  static int max_dyn[MAX_GPUS];
+  static std::once_flag max_dyn_once[MAX_GPUS];
+  std::call_once(max_dyn_once[gpu_index], [gpu_index] {
+    int max_smem = 0;
+    B200_CHECK(cudaDeviceGetAttribute(
+        &max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, (int)gpu_index));
+    cudaFuncAttributes fattr;
+    B200_CHECK(
+        cudaFuncGetAttributes(&fattr, pbs_generic_kernel<256, false, Torus>));
+    max_dyn[gpu_index] = max_smem - (int)fattr.sharedSizeBytes;
   });
-  if (smem > (size_t)max_dyn) {
+  if (smem > (size_t)max_dyn[gpu_index]) {
     // working set larger than one SM's shared memory (N >= 8192 ...): same
     // kernel over a per-CTA slice of a stream-ordered global workspace, a
     // persistent grid striding over the samples
-    int sms = 0;
-    B200_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount,
-                                      (int)gpu_index));
-    const uint32_t grid = std::min<uint32_t>(num_samples, 2u * (uint32_t)sms);
+    const uint32_t grid = std::min(num_samples, 2u * sm_count(gpu_index));
     const size_t stride = (smem + 255) / 256 * 256;
     unsigned char *ws = nullptr;
     B200_CHECK(cudaMallocFromPoolAsync(&ws, stride * grid,
                                        workspace_pool(gpu_index), stream));
-    pbs_generic_kernel<256, true, Torus><<<grid, 256, 0, stream>>>(
-        lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
-        static_cast<const cplx *>(bsk), t.gen_tw[logM], t.gen_root[logM], n, k,
-        N, logM, base_log, l, grouping, num_many_lut, lut_stride, centered_ms,
-        multibit_ties_even().load(), num_samples, ws, stride);
-    B200_CHECK(cudaGetLastError());
-    count_launch();
+    launch(pbs_generic_kernel<256, true, Torus>,
+           {grid, 256, 0, stream, gpu_index}, lwe_out, out_idx, luts, lut_idx,
+           lwe_in, in_idx, static_cast<const cplx *>(bsk), t.gen_tw[logM],
+           t.gen_root[logM], n, k, N, logM, base_log, l, grouping,
+           num_many_lut, lut_stride, centered_ms, multibit_ties_even().load(),
+           num_samples, ws, stride);
     t_last_pbs_kernel = std::is_same<Torus, uint32_t>::value
                             ? "generic_workspace_u32"
                             : "generic_workspace";
     B200_CHECK(cudaFreeAsync(ws, stream));
     return;
   }
-  pbs_generic_kernel<256, false, Torus><<<num_samples, 256, smem, stream>>>(
-      lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
-      static_cast<const cplx *>(bsk), t.gen_tw[logM], t.gen_root[logM], n, k,
-      N, logM, base_log, l, grouping, num_many_lut, lut_stride, centered_ms,
-      multibit_ties_even().load());
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(pbs_generic_kernel<256, false, Torus>,
+         {num_samples, 256, smem, stream, gpu_index, (size_t)max_dyn[gpu_index]},
+         lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
+         static_cast<const cplx *>(bsk), t.gen_tw[logM], t.gen_root[logM], n,
+         k, N, logM, base_log, l, grouping, num_many_lut, lut_stride,
+         centered_ms, multibit_ties_even().load(), 0, nullptr,
+         0); // no workspace
   t_last_pbs_kernel =
       std::is_same<Torus, uint32_t>::value ? "generic_smem_u32" : "generic_smem";
 }
@@ -442,155 +535,15 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
   if (grouping <= 1 && uses_fast_path(n, k, N, l)) {
     B200_PANIC_IF_FALSE(base_log <= 31, "Cuda error (PBS): base_log > 31");
     const DeviceTables &t = device_tables(gpu_index, 0);
-    static std::once_flag attr_once[MAX_GPUS];
-    std::call_once(attr_once[gpu_index], [] {
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22Smem)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v3_kernel<0, 0>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(P22SmemV3)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v3_kernel<0, 1>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(P22SmemV3)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v3_kernel<1, 1>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(P22SmemV3)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v3_kernel<2, 1>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(P22SmemV3)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v3_kernel<3, 1>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV3Tma)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v3_kernel<0, 1, 1>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(P22SmemV3)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<0, false>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<4, false>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<0, true>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<4, true>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<1, true>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<1, true>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<2, true>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<2, true>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<0, true, 1>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<4, true>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<2, true, 1>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<2, true>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<0, true, 2, 1>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<4, true>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<2, true>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<2, true, 2, 2>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<2, true>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<0, true, 2>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<4, true>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<2, true, 2>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<2, true>)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n2048_k1_l1_v6_kernel<2, true, 3>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(P22SmemV6<2, true>)));
-    });
-    auto launch_reg = [&](auto kernel, size_t smem, const char *name) {
-      kernel<<<num_samples, 128, smem, stream>>>(
-          lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
-          static_cast<const cplx *>(bsk), t.fft1024, n, base_log,
-          num_many_lut, lut_stride, centered_ms);
-      t_last_pbs_kernel = name;
-    };
-    const int variant = fast_variant();
-    if (variant == 1 || base_log > 30) {
-      // v1: 64-bit accumulator (A/B measurements and base_log = 31)
-      launch_reg(pbs_n2048_k1_l1_kernel, sizeof(P22Smem), "n2048_v1");
-    } else if (variant == 3) {
-      launch_reg(pbs_n2048_k1_l1_v3_kernel<0, 0>, sizeof(P22SmemV3), "n2048_v3<0,0>"); // round 1
-    } else if (variant == 5) {
-      launch_reg(pbs_n2048_k1_l1_v3_kernel<0, 1>, sizeof(P22SmemV3), "n2048_v3<0,1>");
-    } else if (variant == 4) {
-      launch_reg(pbs_n2048_k1_l1_v3_kernel<1, 1>, sizeof(P22SmemV3), "n2048_v3<1,1>");
-    } else if (variant == 6) {
-      launch_reg(pbs_n2048_k1_l1_v3_kernel<2, 1>, sizeof(P22SmemV3), "n2048_v3<2,1>");
-    } else if (variant == 7) {
-      // TMA ring for the key block: 208 KiB of shared memory, one CTA per SM
-      launch_reg(pbs_n2048_k1_l1_v3_kernel<3, 1>, sizeof(P22SmemV3Tma), "n2048_v3<3,1>");
-    } else if (variant == 8) {
-      // exchange 2 through warp shuffles (x2_shfl.cuh)
-      launch_reg(pbs_n2048_k1_l1_v3_kernel<0, 1, 1>, sizeof(P22SmemV3), "n2048_v3<0,1,1>");
-    } else if (variant == 9) {
-      // v6: shuffle exchange 2 + one-slot TMA key ring, 2 CTAs / SM
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<0, false>, sizeof(P22SmemV6<4, false>),
-                 "n2048_v6<0,false>");
-    } else if (variant == 10) {
-      // v6 with v3's register key prefetch (isolates the ring)
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<1, true>, sizeof(P22SmemV6<1, true>),
-                 "n2048_v6<1,true>");
-    } else if (variant == 11) {
-      // v6 hybrid: own row in registers, other row through the ring
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<2, true>, sizeof(P22SmemV6<2, true>),
-                 "n2048_v6<2,true>");
-    } else if (variant == 14) {
-      // v6 with the switched mask staged in shared memory: one CTA per SM
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<0, true>, sizeof(P22SmemV6<4, true>),
-                 "n2048_v6<0,true>");
-    } else if (variant == 15) {
-      // v6 ring, digits converted through the fp64 ADD pipe instead of I2F
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<0, true, 1>, sizeof(P22SmemV6<4, true>),
-                 "n2048_v6<0,true,1>");
-    } else if (variant == 16) {
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<2, true, 1>, sizeof(P22SmemV6<2, true>),
-                 "n2048_v6<2,true,1>");
-    } else if (variant == 20) {
-      // the shipped two-CTA instance (lane-pair layout, see below)
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1>, sizeof(P22SmemV6<2, true>),
-                 "n2048_v6<2,true,2,1>");
-    } else if (variant == 22) {
-      // v6 hybrid with both CTA barriers of a step split (own-row products before
-      // the wait for the other group's spectrum)
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<2, true, 2, 2>, sizeof(P22SmemV6<2, true>),
-                 "n2048_v6<2,true,2,2>");
-    } else if (variant == 21) {
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<0, true, 2, 1>, sizeof(P22SmemV6<4, true>),
-                 "n2048_v6<0,true,2,1>");
-    } else if (variant == 19) {
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<0, true, 2>, sizeof(P22SmemV6<4, true>),
-                 "n2048_v6<0,true,2>");
-    } else if (variant == 17) {
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<2, true, 2>, sizeof(P22SmemV6<2, true>),
-                 "n2048_v6<2,true,2>");
-    } else if (variant == 18) {
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<2, true, 3>, sizeof(P22SmemV6<2, true>),
-                 "n2048_v6<2,true,3>");
-    } else if (num_samples <= sm_count(gpu_index)) {
+    int variant = fast_variant();
+    if (base_log > 30) {
+      variant = 1; // v1's 64-bit accumulator holds base_log = 31
+    } else if (variant == 0 && num_samples <= sm_count(gpu_index)) {
       // shipped, at most one CTA per SM: v6 with the whole key block of a step
       // through the one-slot TMA ring (no key value is ever waited for) and
       // exchange 2 through warp shuffles
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<0, true, 2>, sizeof(P22SmemV6<4, true>),
-                 "n2048_v6<0,true,2>");
-    } else {
+      variant = 19; // n2048_v6<0,true,2>
+    } else if (variant == 0) {
       // shipped, two CTAs per SM: v6 hybrid -- own key row prefetched into
       // registers, other row (the one v3 waited a full L2 round trip for)
       // through the ring; rotate + decompose with the sign as a predicate
@@ -600,11 +553,14 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
       // the MAC (no spectrum store, no barrier between the polynomials).
       // Bit-identical to variant 17, the same instance in the 64-thread
       // group layout.
-      launch_reg(pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1>, sizeof(P22SmemV6<2, true>),
-                 "n2048_v6<2,true,2,1>");
+      variant = 20; // n2048_v6<2,true,2,1>
     }
-    B200_CHECK(cudaGetLastError());
-    count_launch();
+    const N2048Instance &r = *n2048_instance(variant);
+    launch(r.kernel, {num_samples, 128, r.smem, stream, gpu_index}, lwe_out,
+           out_idx, luts, lut_idx, lwe_in, in_idx,
+           static_cast<const cplx *>(bsk), t.fft1024, n, base_log,
+           num_many_lut, lut_stride, centered_ms);
+    t_last_pbs_kernel = r.name;
     return;
   }
   if (grouping <= 1 && uses_n8192_path(n, k, N, l)) {
@@ -612,18 +568,6 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
                         "Cuda error (PBS): base_log * level_count > 30 is not "
                         "supported for N = 8192");
     const DeviceTables &t = device_tables(gpu_index, 0);
-    static std::once_flag once8k[MAX_GPUS];
-    std::call_once(once8k[gpu_index], [] {
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n8192_k1_l2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(N8192Smem)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n8192_k1_l2_v2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(N8192SmemV2)));
-      B200_CHECK(cudaFuncSetAttribute(
-          pbs_n8192_k1_l2_v2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(N8192SmemV2)));
-    });
     const uint32_t grid = std::min(num_samples, sm_count(gpu_index));
     // per-thread park area of the four spectra of a step (pbs_n8192.cuh)
     cplx *park = nullptr;
@@ -631,10 +575,12 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
                                        workspace_pool(gpu_index), stream));
     // mask bit 2: the first-generation kernel (per-thread key loads), for A/B
     if (register_kernel_mask().load() & 4) {
-      pbs_n8192_k1_l2_kernel<<<grid, 256, sizeof(N8192Smem), stream>>>(
-          lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
-          static_cast<const cplx *>(bsk), t.fft4096, n, base_log, num_samples,
-          num_many_lut, lut_stride, centered_ms, multibit_ties_even().load(), park);
+      launch(pbs_n8192_k1_l2_kernel,
+             {grid, 256, sizeof(N8192Smem), stream, gpu_index}, lwe_out,
+             out_idx, luts, lut_idx, lwe_in, in_idx,
+             static_cast<const cplx *>(bsk), t.fft4096, n, base_log,
+             num_samples, num_many_lut, lut_stride, centered_ms,
+             multibit_ties_even().load(), park);
       t_last_pbs_kernel = "n8192_v1";
     } else {
       static const uint32_t stagger = [] {
@@ -644,17 +590,15 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
       // mask bit 3: the racecheck instance (every thread arrives on the ring's
       // `empty` barriers itself)
       const bool racecheck = register_kernel_mask().load() & 8;
-      auto kernel = racecheck ? pbs_n8192_k1_l2_v2_kernel<true>
-                              : pbs_n8192_k1_l2_v2_kernel<false>;
-      kernel<<<grid, 256, sizeof(N8192SmemV2), stream>>>(
-          lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
-          static_cast<const cplx *>(bsk), t.fft4096, n, base_log, num_samples,
-          num_many_lut, lut_stride, centered_ms, multibit_ties_even().load(),
-          stagger, park);
+      launch(racecheck ? pbs_n8192_k1_l2_v2_kernel<true>
+                       : pbs_n8192_k1_l2_v2_kernel<false>,
+             {grid, 256, sizeof(N8192SmemV2), stream, gpu_index}, lwe_out,
+             out_idx, luts, lut_idx, lwe_in, in_idx,
+             static_cast<const cplx *>(bsk), t.fft4096, n, base_log,
+             num_samples, num_many_lut, lut_stride, centered_ms,
+             multibit_ties_even().load(), stagger, park);
       t_last_pbs_kernel = racecheck ? "n8192_v2<true>" : "n8192_v2<false>";
     }
-    B200_CHECK(cudaGetLastError());
-    count_launch();
     B200_CHECK(cudaFreeAsync(park, stream));
     return;
   }
@@ -665,68 +609,45 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
     // per CTA by launch size; 2 / 3: ring with two / one LWE per CTA; 4: ring with
     // three; 1: register key ring, two LWEs per CTA, two CTAs per SM
     const int mode512 = n512_mode_sel().load();
-    static std::once_flag once512[MAX_GPUS];
-    auto set_attr = [](auto kernel, size_t smem) {
-      B200_CHECK(cudaFuncSetAttribute(
-          kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    };
-    std::call_once(once512[gpu_index], [&] {
-      set_attr(pbs_n512_kernel<1, 2, false>, sizeof(N512Smem<1, 2, false>));
-      set_attr(pbs_n512_kernel<2, 2, false>, sizeof(N512Smem<2, 2, false>));
-      set_attr(pbs_n512_kernel<3, 2, false>, sizeof(N512Smem<3, 2, false>));
-      set_attr(pbs_n512_kernel<4, 2, false>, sizeof(N512Smem<4, 2, false>));
-      set_attr(pbs_n512_kernel<1, 2, true>, sizeof(N512Smem<1, 2, true>));
-      set_attr(pbs_n512_kernel<2, 2, true>, sizeof(N512Smem<2, 2, true>));
-      set_attr(pbs_n512_kernel<3, 2, true>, sizeof(N512Smem<3, 2, true>));
-      set_attr(pbs_n512_kernel<4, 2, true>, sizeof(N512Smem<4, 2, true>));
-      set_attr(pbs_n512_kernel<1, 1, true>, sizeof(N512Smem<1, 1, true>));
-      set_attr(pbs_n512_kernel<2, 1, true>, sizeof(N512Smem<2, 1, true>));
-      set_attr(pbs_n512_kernel<3, 1, true>, sizeof(N512Smem<3, 1, true>));
-      set_attr(pbs_n512_kernel<4, 1, true>, sizeof(N512Smem<4, 1, true>));
-      set_attr(pbs_n512_kernel<1, 3, true>, sizeof(N512Smem<1, 3, true>));
-      set_attr(pbs_n512_kernel<2, 3, true>, sizeof(N512Smem<2, 3, true>));
-      set_attr(pbs_n512_kernel<3, 3, true>, sizeof(N512Smem<3, 3, true>));
-      set_attr(pbs_n512_kernel<4, 3, true>, sizeof(N512Smem<4, 3, true>));
-    });
-    auto launch512 = [&](auto kernel, size_t smem, uint32_t G, uint32_t ctas_per_sm,
-                         const char *name) {
-      // persistent grid (see the kernel)
-      const uint32_t groups = (num_samples + G - 1) / G;
-      const uint32_t grid = std::min(groups, ctas_per_sm * sm_count(gpu_index));
-      kernel<<<grid, 16 * (k + 1) * G, smem, stream>>>(
-          lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
-          static_cast<const cplx *>(bsk), t.fft256, n, base_log, num_samples,
-          num_many_lut, lut_stride, centered_ms);
-      t_last_pbs_kernel = name;
-    };
     // automatic: the fewest LWEs per CTA that still covers the launch in one
     // round of the persistent grid (latency), three per CTA beyond that
     // (throughput)
     const uint32_t sms = sm_count(gpu_index);
     const int per_cta = mode512 == 3 ? 1 : mode512 == 2 ? 2 : mode512 == 0 && num_samples <= sms ? 1
                         : mode512 == 0 && num_samples <= 2 * sms ? 2 : 3;
-#define B200_LAUNCH512(K)                                                       \
-  if (mode512 == 1)                                                             \
-    launch512(pbs_n512_kernel<K, 2, false>, sizeof(N512Smem<K, 2, false>), 2, 2, \
-              "n512<" #K ",2,false>");                                          \
-  else if (per_cta == 1)                                                        \
-    launch512(pbs_n512_kernel<K, 1, true>, sizeof(N512Smem<K, 1, true>), 1, 1,  \
-              "n512<" #K ",1,true>");                                           \
-  else if (per_cta == 2)                                                        \
-    launch512(pbs_n512_kernel<K, 2, true>, sizeof(N512Smem<K, 2, true>), 2, 1,  \
-              "n512<" #K ",2,true>");                                           \
-  else                                                                          \
-    launch512(pbs_n512_kernel<K, 3, true>, sizeof(N512Smem<K, 3, true>), 3, 1,  \
-              "n512<" #K ",3,true>")
-    switch (k) {
-    case 1: B200_LAUNCH512(1); break;
-    case 2: B200_LAUNCH512(2); break;
-    case 3: B200_LAUNCH512(3); break;
-    default: B200_LAUNCH512(4); break;
-    }
-#undef B200_LAUNCH512
-    B200_CHECK(cudaGetLastError());
-    count_launch();
+    // [k - 1][0: register key ring, two LWEs per CTA, two CTAs per SM;
+    //         G = 1, 2, 3: TMA key ring, G LWEs per CTA, one CTA per SM]
+    static const struct {
+      decltype(&pbs_n512_kernel<1, 1, true>) kernel;
+      size_t smem;
+      const char *name;
+    } n512_instances[4][4] = {
+        {{pbs_n512_kernel<1, 2, false>, sizeof(N512Smem<1, 2, false>), "n512<1,2,false>"},
+         {pbs_n512_kernel<1, 1, true>, sizeof(N512Smem<1, 1, true>), "n512<1,1,true>"},
+         {pbs_n512_kernel<1, 2, true>, sizeof(N512Smem<1, 2, true>), "n512<1,2,true>"},
+         {pbs_n512_kernel<1, 3, true>, sizeof(N512Smem<1, 3, true>), "n512<1,3,true>"}},
+        {{pbs_n512_kernel<2, 2, false>, sizeof(N512Smem<2, 2, false>), "n512<2,2,false>"},
+         {pbs_n512_kernel<2, 1, true>, sizeof(N512Smem<2, 1, true>), "n512<2,1,true>"},
+         {pbs_n512_kernel<2, 2, true>, sizeof(N512Smem<2, 2, true>), "n512<2,2,true>"},
+         {pbs_n512_kernel<2, 3, true>, sizeof(N512Smem<2, 3, true>), "n512<2,3,true>"}},
+        {{pbs_n512_kernel<3, 2, false>, sizeof(N512Smem<3, 2, false>), "n512<3,2,false>"},
+         {pbs_n512_kernel<3, 1, true>, sizeof(N512Smem<3, 1, true>), "n512<3,1,true>"},
+         {pbs_n512_kernel<3, 2, true>, sizeof(N512Smem<3, 2, true>), "n512<3,2,true>"},
+         {pbs_n512_kernel<3, 3, true>, sizeof(N512Smem<3, 3, true>), "n512<3,3,true>"}},
+        {{pbs_n512_kernel<4, 2, false>, sizeof(N512Smem<4, 2, false>), "n512<4,2,false>"},
+         {pbs_n512_kernel<4, 1, true>, sizeof(N512Smem<4, 1, true>), "n512<4,1,true>"},
+         {pbs_n512_kernel<4, 2, true>, sizeof(N512Smem<4, 2, true>), "n512<4,2,true>"},
+         {pbs_n512_kernel<4, 3, true>, sizeof(N512Smem<4, 3, true>), "n512<4,3,true>"}}};
+    const int col = mode512 == 1 ? 0 : per_cta;
+    const auto &r = n512_instances[k - 1][col];
+    const uint32_t G = col ? col : 2, ctas_per_sm = col ? 1 : 2;
+    // persistent grid (see the kernel)
+    const uint32_t grid = std::min((num_samples + G - 1) / G, ctas_per_sm * sms);
+    launch(r.kernel, {grid, 16 * (k + 1) * G, r.smem, stream, gpu_index},
+           lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
+           static_cast<const cplx *>(bsk), t.fft256, n, base_log, num_samples,
+           num_many_lut, lut_stride, centered_ms);
+    t_last_pbs_kernel = r.name;
     return;
   }
   if (grouping > 1 && uses_multibit_fast_path(k, N, l, grouping)) {
@@ -737,22 +658,6 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
                         "Cuda error (multi-bit PBS): base_log * level_count "
                         "> 31 is not supported for N = 2048, k = 1");
     const DeviceTables &t = device_tables(gpu_index, 10);
-    static std::once_flag mb_once[MAX_GPUS];
-    auto for_each_instance = [&](auto &&fn) {
-      fn(pbs_multibit_n2048_k1_kernel<2, 1>, 2u, 1u, "multibit_fused<2,1>");
-      fn(pbs_multibit_n2048_k1_kernel<2, 2>, 2u, 2u, "multibit_fused<2,2>");
-      fn(pbs_multibit_n2048_k1_kernel<3, 1>, 3u, 1u, "multibit_fused<3,1>");
-      fn(pbs_multibit_n2048_k1_kernel<3, 2>, 3u, 2u, "multibit_fused<3,2>");
-      fn(pbs_multibit_n2048_k1_kernel<4, 1>, 4u, 1u, "multibit_fused<4,1>");
-      fn(pbs_multibit_n2048_k1_kernel<4, 2>, 4u, 2u, "multibit_fused<4,2>");
-    };
-    std::call_once(mb_once[gpu_index], [&] {
-      for_each_instance([](auto kernel, uint32_t, uint32_t, const char *) {
-        B200_CHECK(cudaFuncSetAttribute(
-            kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-            (int)sizeof(MbSmem)));
-      });
-    });
     // low-latency mode for launches that cannot fill the GPU with the fused
     // kernel: bundle for all groups at once, then the sequential products
     if (num_samples <= multibit_ll_max_samples(gpu_index)) {
@@ -762,18 +667,24 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
                          lut_stride);
       return;
     }
-    for_each_instance([&](auto kernel, uint32_t kg, uint32_t kl, const char *name) {
-      if (kg != grouping || kl != l)
-        return;
-      kernel<<<num_samples, 128, sizeof(MbSmem), stream>>>(
-          lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
-          static_cast<const cplx *>(bsk), t.fft1024, t.gen_root[10],
-          t.mono2048, n, base_log, num_many_lut, lut_stride,
-          multibit_ties_even().load());
-      t_last_pbs_kernel = name;
-    });
-    B200_CHECK(cudaGetLastError());
-    count_launch();
+    // [grouping - 2][l - 1]
+    static const struct {
+      decltype(&pbs_multibit_n2048_k1_kernel<2, 1>) kernel;
+      const char *name;
+    } fused_instances[3][2] = {
+        {{pbs_multibit_n2048_k1_kernel<2, 1>, "multibit_fused<2,1>"},
+         {pbs_multibit_n2048_k1_kernel<2, 2>, "multibit_fused<2,2>"}},
+        {{pbs_multibit_n2048_k1_kernel<3, 1>, "multibit_fused<3,1>"},
+         {pbs_multibit_n2048_k1_kernel<3, 2>, "multibit_fused<3,2>"}},
+        {{pbs_multibit_n2048_k1_kernel<4, 1>, "multibit_fused<4,1>"},
+         {pbs_multibit_n2048_k1_kernel<4, 2>, "multibit_fused<4,2>"}}};
+    const auto &r = fused_instances[grouping - 2][l - 1];
+    launch(r.kernel, {num_samples, 128, sizeof(MbSmem), stream, gpu_index},
+           lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
+           static_cast<const cplx *>(bsk), t.fft1024, t.gen_root[10],
+           t.mono2048, n, base_log, num_many_lut, lut_stride,
+           multibit_ties_even().load());
+    t_last_pbs_kernel = r.name;
     return;
   }
   if (grouping > 1) {
@@ -789,65 +700,59 @@ static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
 
 // standard-domain BSK (device staging buffer) -> Fourier BSK in the engine's
 // layout
+template <typename Torus>
 static void convert_bsk_staged(cudaStream_t stream, uint32_t gpu_index,
-                               void *dest, const uint64_t *staging, uint32_t k,
+                               void *dest, const Torus *staging, uint32_t k,
                                uint32_t N, uint32_t l, uint32_t num_ggsw,
                                bool fast_layout, uint32_t multibit_grouping) {
   const uint32_t logM = ilog2_exact(N) - 1;
   const size_t polys = (size_t)num_ggsw * l * (k + 1) * (k + 1);
   const DeviceTables &t = device_tables(gpu_index, fast_layout ? 0 : logM);
-  if (multibit_grouping) {
-    bsk_convert_multibit_n2048_kernel<<<(unsigned)polys, 64, 0, stream>>>(
-        static_cast<cplx *>(dest), staging, t.fft1024, l, multibit_grouping);
-  } else if (fast_layout) {
-    bsk_convert_n2048_k1_l1_kernel<<<(unsigned)polys, 64, 0, stream>>>(
-        static_cast<cplx *>(dest), staging, t.fft1024);
-  } else if (uses_n8192_path(num_ggsw, k, N, l)) {
-    static std::once_flag conv8k_once[MAX_GPUS];
-    std::call_once(conv8k_once[gpu_index], [] {
-      B200_CHECK(cudaFuncSetAttribute(
-          bsk_convert_n8192_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)(P8K_M * sizeof(cplx))));
-    });
-    bsk_convert_n8192_kernel<<<(unsigned)polys, 256, P8K_M * sizeof(cplx),
-                               stream>>>(static_cast<cplx *>(dest), staging,
-                                         t.fft4096);
-  } else if (uses_n512_path(num_ggsw, k, N, l)) {
-    bsk_convert_n512_kernel<<<(unsigned)((polys + 1) / 2), 32, 0, stream>>>(
-        static_cast<cplx *>(dest), staging, t.fft256, k + 1, (uint32_t)polys);
-  } else {
-    static std::once_flag conv_once[MAX_GPUS];
-    std::call_once(conv_once[gpu_index], [] {
-      B200_CHECK(cudaFuncSetAttribute(
-          bsk_convert_generic_kernel<uint64_t>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 / 2 * 16));
-      B200_CHECK(cudaFuncSetAttribute(
-          bsk_convert_generic_kernel<uint32_t>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 / 2 * 16));
-    });
-    bsk_convert_generic_kernel<uint64_t>
-        <<<(unsigned)polys, 256, (N / 2) * sizeof(cplx), stream>>>(
-            static_cast<cplx *>(dest), staging, t.gen_tw[logM], N, logM);
-  }
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  cplx *out = static_cast<cplx *>(dest);
+  // limit: the shared memory of the largest N, 16384
+  const auto generic = [&] {
+    launch(bsk_convert_generic_kernel<Torus>,
+           {(unsigned)polys, 256, (N / 2) * sizeof(cplx), stream, gpu_index,
+            (16384 / 2) * sizeof(cplx)},
+           out, staging, t.gen_tw[logM], N, logM);
+  };
+  if constexpr (std::is_same<Torus, uint32_t>::value)
+    generic(); // the only layout of the 32-bit torus
+  else if (multibit_grouping)
+    launch(bsk_convert_multibit_n2048_kernel,
+           {(unsigned)polys, 64, 0, stream, gpu_index}, out, staging,
+           t.fft1024, l, multibit_grouping);
+  else if (fast_layout)
+    launch(bsk_convert_n2048_k1_l1_kernel,
+           {(unsigned)polys, 64, 0, stream, gpu_index}, out, staging,
+           t.fft1024);
+  else if (uses_n8192_path(num_ggsw, k, N, l))
+    launch(bsk_convert_n8192_kernel,
+           {(unsigned)polys, 256, P8K_M * sizeof(cplx), stream, gpu_index},
+           out, staging, t.fft4096);
+  else if (uses_n512_path(num_ggsw, k, N, l))
+    launch(bsk_convert_n512_kernel,
+           {(unsigned)((polys + 1) / 2), 32, 0, stream, gpu_index}, out,
+           staging, t.fft256, k + 1, (uint32_t)polys);
+  else
+    generic();
 }
 
 // host standard-domain BSK -> device Fourier BSK in the engine's layout
+template <typename Torus>
 static void convert_bsk(cudaStream_t stream, uint32_t gpu_index, void *dest,
-                        const void *src_host, uint32_t n, uint32_t k,
-                        uint32_t N, uint32_t l, uint32_t num_ggsw,
-                        bool fast_layout, uint32_t multibit_grouping = 0) {
-  (void)n;
+                        const void *src_host, uint32_t k, uint32_t N,
+                        uint32_t l, uint32_t num_ggsw, bool fast_layout,
+                        uint32_t multibit_grouping = 0) {
   check_polynomial_size(N);
   const size_t polys = (size_t)num_ggsw * l * (k + 1) * (k + 1);
-  const size_t bytes = polys * N * sizeof(uint64_t);
-  uint64_t *staging = nullptr;
+  const size_t bytes = polys * N * sizeof(Torus);
+  Torus *staging = nullptr;
   B200_CHECK(cudaMallocAsync(&staging, bytes, stream));
   B200_CHECK(cudaMemcpyAsync(staging, src_host, bytes, cudaMemcpyHostToDevice,
                              stream));
-  convert_bsk_staged(stream, gpu_index, dest, staging, k, N, l, num_ggsw,
-                     fast_layout, multibit_grouping);
+  convert_bsk_staged<Torus>(stream, gpu_index, dest, staging, k, N, l,
+                            num_ggsw, fast_layout, multibit_grouping);
   B200_CHECK(cudaFreeAsync(staging, stream));
 }
 
@@ -893,11 +798,10 @@ static void oprf_expand(cudaStream_t stream, uint32_t gpu_index,
   const uint64_t last_start = first_byte + width * ((uint64_t)n * num_blocks - 1);
   const uint64_t ctas = last_start / (16 * OPRF_OWNED_BLOCKS) + 1;
   B200_PANIC_IF_FALSE(ctas < (1ull << 31), "Cuda error (OPRF): batch too large");
-  oprf_expand_kernel<<<(unsigned)ctas, OPRF_THREADS, 0, stream>>>(
-      lwe_out, tables, key, ctr_lo, ctr_hi, (uint32_t)first_byte, n,
-      num_blocks, log_modulus);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(oprf_expand_kernel,
+         {(unsigned)ctas, OPRF_THREADS, 0, stream, gpu_index}, lwe_out, tables,
+         key, ctr_lo, ctr_hi, (uint32_t)first_byte, n, num_blocks,
+         log_modulus);
 }
 
 // seeded BSK (host bodies + AES-CTR mask seed) -> device Fourier BSK
@@ -924,11 +828,9 @@ static void convert_seeded_bsk(cudaStream_t stream, uint32_t gpu_index,
   B200_CHECK(cudaMallocAsync(&bodies, body_bytes, stream));
   B200_CHECK(cudaMemcpyAsync(bodies, bodies_host, body_bytes,
                              cudaMemcpyHostToDevice, stream));
-  seeded_bsk_expand_kernel<<<sm_count(gpu_index) * 8, 256, 0, stream>>>(
-      staging, bodies, tables, key, ctr_lo, ctr_hi,
-      first_byte_index / 8, rows, k, N);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(seeded_bsk_expand_kernel,
+         {sm_count(gpu_index) * 8, 256, 0, stream, gpu_index}, staging, bodies,
+         tables, key, ctr_lo, ctr_hi, first_byte_index / 8, rows, k, N);
   convert_bsk_staged(stream, gpu_index, dest, staging, k, N, l, num_ggsw,
                      fast_layout, multibit_grouping);
   B200_CHECK(cudaFreeAsync(bodies, stream));
@@ -1010,10 +912,8 @@ static void compact_expand(cudaStream_t st, uint32_t gpu_index,
   const uint64_t words = max_count * (n + 1);
   const dim3 grid((unsigned)((words + EXPAND_THREADS - 1) / EXPAND_THREADS),
                   std::min<uint32_t>(num_lists, 65535u));
-  compact_expand_kernel<<<grid, EXPAND_THREADS, 0, st>>>(lwe_out, lists_in,
-                                                         d_descs, num_lists, n);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(compact_expand_kernel, {grid, EXPAND_THREADS, 0, st, gpu_index},
+         lwe_out, lists_in, d_descs, num_lists, n);
   B200_CHECK(cudaFreeAsync(d_descs, st));
 }
 
@@ -1086,23 +986,17 @@ static void cpk_encrypt_zeros(cudaStream_t st, uint32_t gpu_index,
   B200_CHECK(cudaMemcpyAsync(ws + state_bytes, staging.data(), staging.size(),
                              cudaMemcpyHostToDevice, st));
   const AesTables *tables = aes_device_tables(gpu_index);
-  rerand_seed_init_kernel<<<(num_seeds + 255) / 256, 256, 0, st>>>(
-      d_states, d_seeds, tables, num_seeds);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
-  static std::once_flag smem_once[MAX_GPUS];
-  std::call_once(smem_once[gpu_index], [] {
-    B200_CHECK(cudaFuncSetAttribute(rerand_zeros_kernel,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)rerand_smem_bytes(16384)));
-  });
+  launch(rerand_seed_init_kernel,
+         {(num_seeds + 255) / 256, 256, 0, st, gpu_index}, d_states, d_seeds,
+         tables, num_seeds);
   const uint64_t tiles = n / RERAND_THREADS +
                          (max_count + RERAND_THREADS - 1) / RERAND_THREADS;
   const dim3 grid((unsigned)tiles, std::min<uint32_t>(num_bins, 65535u));
-  rerand_zeros_kernel<<<grid, RERAND_THREADS, rerand_smem_bytes(n), st>>>(
-      out, cpk, d_states, d_descs, tables, num_bins, n, bound_log2, accumulate);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(rerand_zeros_kernel,
+         {grid, RERAND_THREADS, rerand_smem_bytes(n), st, gpu_index,
+          rerand_smem_bytes(16384)},
+         out, cpk, d_states, d_descs, tables, num_bins, n, bound_log2,
+         accumulate);
   B200_CHECK(cudaFreeAsync(ws, st));
 }
 
@@ -1283,11 +1177,10 @@ void cuda_convert_lwe_programmable_bootstrap_key_64_async(
     uint32_t input_lwe_dim, uint32_t glwe_dim, uint32_t level_count,
     uint32_t polynomial_size) {
   set_device(gpu_index);
-  convert_bsk(static_cast<cudaStream_t>(stream), gpu_index, dest, src,
-              input_lwe_dim, glwe_dim, polynomial_size, level_count,
-              input_lwe_dim,
-              uses_fast_path(input_lwe_dim, glwe_dim, polynomial_size,
-                             level_count));
+  convert_bsk<uint64_t>(static_cast<cudaStream_t>(stream), gpu_index, dest, src,
+                        glwe_dim, polynomial_size, level_count, input_lwe_dim,
+                        uses_fast_path(input_lwe_dim, glwe_dim,
+                                       polynomial_size, level_count));
 }
 
 uint64_t scratch_cuda_programmable_bootstrap_64_async(
@@ -1329,14 +1222,9 @@ void cuda_programmable_bootstrap_64_async(
     uint32_t polynomial_size, uint32_t base_log, uint32_t level_count,
     uint32_t num_samples, uint32_t num_many_lut, uint32_t lut_stride) {
   set_device(gpu_index);
-  const PbsScratch *s = reinterpret_cast<const PbsScratch *>(buffer);
-  B200_PANIC_IF_FALSE(s && s->magic == SCRATCH_MAGIC && s->type == CLASSICAL,
-                      "Cuda error (classical PBS): invalid scratch buffer");
-  B200_PANIC_IF_FALSE(
-      s->glwe_dim == glwe_dimension && s->poly_size == polynomial_size &&
-          s->level_count == level_count,
-      "Cuda error (classical PBS): scratch buffer was created for other "
-      "parameters");
+  const PbsScratch &s =
+      pbs_scratch(buffer, CLASSICAL, "classical PBS",
+                  PbsShape{glwe_dimension, polynomial_size, level_count});
   B200_PANIC_IF_FALSE(base_log <= 64,
                       "Cuda error (classical PBS): base log should be <= 64");
   launch_pbs(static_cast<cudaStream_t>(stream), gpu_index,
@@ -1348,7 +1236,7 @@ void cuda_programmable_bootstrap_64_async(
              static_cast<const uint64_t *>(lwe_input_indexes),
              bootstrapping_key, lwe_dimension, glwe_dimension, polynomial_size,
              base_log, level_count, 1, num_samples, num_many_lut, lut_stride,
-             s->centered_ms);
+             s.centered_ms);
 }
 
 void cleanup_cuda_programmable_bootstrap_64(void *stream, uint32_t gpu_index,
@@ -1377,29 +1265,9 @@ void cuda_convert_lwe_programmable_bootstrap_key_32_async(
     uint32_t input_lwe_dim, uint32_t glwe_dim, uint32_t level_count,
     uint32_t polynomial_size) {
   set_device(gpu_index);
-  check_polynomial_size(polynomial_size);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const uint32_t logM = ilog2_exact(polynomial_size) - 1;
-  const size_t polys =
-      (size_t)input_lwe_dim * level_count * (glwe_dim + 1) * (glwe_dim + 1);
-  const size_t bytes = polys * polynomial_size * sizeof(uint32_t);
-  const DeviceTables &t = device_tables(gpu_index, logM);
-  uint32_t *staging = nullptr;
-  B200_CHECK(cudaMallocAsync(&staging, bytes, st));
-  B200_CHECK(cudaMemcpyAsync(staging, src, bytes, cudaMemcpyHostToDevice, st));
-  static std::once_flag once[MAX_GPUS];
-  std::call_once(once[gpu_index], [] {
-    B200_CHECK(cudaFuncSetAttribute(
-        bsk_convert_generic_kernel<uint32_t>,
-        cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 / 2 * 16));
-  });
-  bsk_convert_generic_kernel<uint32_t>
-      <<<(unsigned)polys, 256, (polynomial_size / 2) * sizeof(cplx), st>>>(
-          static_cast<cplx *>(dest), staging, t.gen_tw[logM], polynomial_size,
-          logM);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
-  B200_CHECK(cudaFreeAsync(staging, st));
+  convert_bsk<uint32_t>(static_cast<cudaStream_t>(stream), gpu_index, dest, src,
+                        glwe_dim, polynomial_size, level_count, input_lwe_dim,
+                        false);
 }
 
 void cuda_programmable_bootstrap_lwe_ciphertext_vector_32_async(
@@ -1411,9 +1279,7 @@ void cuda_programmable_bootstrap_lwe_ciphertext_vector_32_async(
     uint32_t polynomial_size, uint32_t base_log, uint32_t level_count,
     uint32_t num_samples, uint32_t num_many_lut, uint32_t lut_stride) {
   set_device(gpu_index);
-  const PbsScratch *s = reinterpret_cast<const PbsScratch *>(buffer);
-  B200_PANIC_IF_FALSE(s && s->magic == SCRATCH_MAGIC && s->type == CLASSICAL,
-                      "Cuda error (classical PBS): invalid scratch buffer");
+  const PbsScratch &s = pbs_scratch(buffer, CLASSICAL, "classical PBS");
   B200_PANIC_IF_FALSE(base_log <= 32,
                       "Cuda error (classical PBS): base log should be <= 32");
   if (num_samples == 0)
@@ -1428,7 +1294,7 @@ void cuda_programmable_bootstrap_lwe_ciphertext_vector_32_async(
       static_cast<const uint32_t *>(lwe_array_in),
       static_cast<const uint32_t *>(lwe_input_indexes), bootstrapping_key,
       lwe_dimension, glwe_dimension, polynomial_size, base_log, level_count, 1,
-      num_samples, num_many_lut ? num_many_lut : 1, lut_stride, s->centered_ms);
+      num_samples, num_many_lut ? num_many_lut : 1, lut_stride, s.centered_ms);
 }
 
 // ===========================================================================
@@ -1460,9 +1326,9 @@ void cuda_convert_lwe_multi_bit_programmable_bootstrap_key_64_async(
   const bool mb_fast = grouping_factor >= 2 &&
                        uses_multibit_fast_path(glwe_dim, polynomial_size,
                                                level_count, grouping_factor);
-  convert_bsk(static_cast<cudaStream_t>(stream), gpu_index, dest, src,
-              input_lwe_dim, glwe_dim, polynomial_size, level_count, num_ggsw,
-              mb_fast, mb_fast ? grouping_factor : 0);
+  convert_bsk<uint64_t>(static_cast<cudaStream_t>(stream), gpu_index, dest, src,
+                        glwe_dim, polynomial_size, level_count, num_ggsw,
+                        mb_fast, mb_fast ? grouping_factor : 0);
 }
 
 void b200_convert_seeded_lwe_programmable_bootstrap_key_64_async(
@@ -1526,9 +1392,7 @@ void cuda_multi_bit_programmable_bootstrap_64_async(
     uint32_t level_count, uint32_t num_samples, uint32_t num_many_lut,
     uint32_t lut_stride) {
   set_device(gpu_index);
-  const PbsScratch *s = reinterpret_cast<const PbsScratch *>(buffer);
-  B200_PANIC_IF_FALSE(s && s->magic == SCRATCH_MAGIC && s->type == MULTI_BIT,
-                      "Cuda error (multi-bit PBS): invalid scratch buffer");
+  pbs_scratch(buffer, MULTI_BIT, "multi-bit PBS");
   B200_PANIC_IF_FALSE(base_log <= 64,
                       "Cuda error (multi-bit PBS): base log should be <= 64");
   B200_PANIC_IF_FALSE(grouping_factor >= 2,
@@ -1595,6 +1459,7 @@ static void keyswitch_64(void *stream, uint32_t gpu_index, void *lwe_array_out,
   set_device(gpu_index);
   if (num_samples == 0)
     return;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   B200_PANIC_IF_FALSE(level_count >= 1 && level_count <= 32 && base_log >= 1 &&
                           base_log * level_count <= 63,
                       "Cuda error (keyswitch): unsupported decomposition "
@@ -1610,16 +1475,6 @@ static void keyswitch_64(void *stream, uint32_t gpu_index, void *lwe_array_out,
   const bool imma_exact =
       base_log <= 7 && terms * 255ull * (1ull << (base_log - 1)) < (1ull << 31);
   if (!force_int && imma_exact && (ks_path.empty() || ks_path == "imma")) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    static std::once_flag ki_once[MAX_GPUS];
-    std::call_once(ki_once[gpu_index], [] {
-      B200_CHECK(cudaFuncSetAttribute(
-          keyswitch_imma_kernel<1>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize, KiCfg<1>::SMEM));
-      B200_CHECK(cudaFuncSetAttribute(
-          keyswitch_imma_kernel<2>,
-          cudaFuncAttributeMaxDynamicSharedMemorySize, KiCfg<2>::SMEM));
-    });
     static const bool wide = std::getenv("B200_KS_IMMA_NB2") != nullptr;
     const uint32_t rows_pad = (num_samples + KI_BM - 1) / KI_BM * KI_BM;
     const uint32_t k_pad = (uint32_t)((terms + KI_BK - 1) / KI_BK * KI_BK);
@@ -1629,31 +1484,32 @@ static void keyswitch_64(void *stream, uint32_t gpu_index, void *lwe_array_out,
     B200_CHECK(cudaMallocFromPoolAsync(&digits, (size_t)rows_pad * k_pad,
                                        workspace_pool(gpu_index), st));
     B200_CHECK(cudaMemsetAsync(digits, 0, (size_t)rows_pad * k_pad, st));
-    ks_digits_kernel<<<dim3(num_samples, (lwe_dimension_in + 255) / 256), 256,
-                       0, st>>>(
-        digits, static_cast<const uint64_t *>(lwe_array_in),
-        static_cast<const uint64_t *>(lwe_input_indexes), lwe_dimension_in,
-        base_log, level_count, k_pad);
-    B200_CHECK(cudaGetLastError());
-    count_launch();
+    launch(ks_digits_kernel,
+           {dim3(num_samples, (lwe_dimension_in + 255) / 256), 256, 0, st,
+            gpu_index},
+           digits, static_cast<const uint64_t *>(lwe_array_in),
+           static_cast<const uint64_t *>(lwe_input_indexes), lwe_dimension_in,
+           base_log, level_count, k_pad);
+    static const struct {
+      decltype(&keyswitch_imma_kernel<1>) kernel;
+      uint32_t bn;
+      size_t smem;
+      const char *name;
+    } imma_instances[2] = {
+        {keyswitch_imma_kernel<1>, KiCfg<1>::BN, KiCfg<1>::SMEM, "ks_imma<1>"},
+        {keyswitch_imma_kernel<2>, KiCfg<2>::BN, KiCfg<2>::SMEM, "ks_imma<2>"}};
+    const auto &r = imma_instances[wide];
     const uint32_t n_bytes = out_len * 8;
-    auto launch = [&](auto kernel, int bn, int smem) {
-      kernel<<<dim3(rows_pad / KI_BM, (n_bytes + bn - 1) / bn), KI_THREADS,
-               smem, st>>>(
-          static_cast<uint64_t *>(lwe_array_out),
-          static_cast<const uint64_t *>(lwe_output_indexes),
-          static_cast<const uint64_t *>(lwe_array_in),
-          static_cast<const uint64_t *>(lwe_input_indexes),
-          static_cast<const uint8_t *>(ksk), digits, lwe_dimension_in,
-          out_len, body_pos, level_count, k_pad, num_samples);
-    };
-    if (wide)
-      launch(keyswitch_imma_kernel<2>, KiCfg<2>::BN, KiCfg<2>::SMEM);
-    else
-      launch(keyswitch_imma_kernel<1>, KiCfg<1>::BN, KiCfg<1>::SMEM);
-    B200_CHECK(cudaGetLastError());
-    count_launch();
-    t_last_ks_kernel = wide ? "ks_imma<2>" : "ks_imma<1>";
+    launch(r.kernel,
+           {dim3(rows_pad / KI_BM, (n_bytes + r.bn - 1) / r.bn), KI_THREADS,
+            r.smem, st, gpu_index},
+           static_cast<uint64_t *>(lwe_array_out),
+           static_cast<const uint64_t *>(lwe_output_indexes),
+           static_cast<const uint64_t *>(lwe_array_in),
+           static_cast<const uint64_t *>(lwe_input_indexes),
+           static_cast<const uint8_t *>(ksk), digits, lwe_dimension_in, out_len,
+           body_pos, level_count, k_pad, num_samples);
+    t_last_ks_kernel = r.name;
     B200_CHECK(cudaFreeAsync(digits, st));
     return;
   }
@@ -1665,38 +1521,26 @@ static void keyswitch_64(void *stream, uint32_t gpu_index, void *lwe_array_out,
   // a pinned path whose precondition fails falls through in the order
   // imma -> f64 -> integer, like the automatic choice
   if (!force_int && (base_log - 1) + 32 + terms_log2 <= 52) {
-    static std::once_flag ks_once[MAX_GPUS];
-    std::call_once(ks_once[gpu_index], [] {
-      B200_CHECK(cudaFuncSetAttribute(
-          keyswitch_f64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-          (int)sizeof(KsfSmem)));
-    });
-    keyswitch_f64_kernel<<<grid, 256, sizeof(KsfSmem),
-                           static_cast<cudaStream_t>(stream)>>>(
-        static_cast<uint64_t *>(lwe_array_out),
-        static_cast<const uint64_t *>(lwe_output_indexes),
-        static_cast<const uint64_t *>(lwe_array_in),
-        static_cast<const uint64_t *>(lwe_input_indexes),
-        static_cast<const uint64_t *>(ksk), lwe_dimension_in, out_len,
-        body_pos, base_log, level_count, num_samples);
-    B200_CHECK(cudaGetLastError());
-    count_launch();
+    launch(keyswitch_f64_kernel, {grid, 256, sizeof(KsfSmem), st, gpu_index},
+           static_cast<uint64_t *>(lwe_array_out),
+           static_cast<const uint64_t *>(lwe_output_indexes),
+           static_cast<const uint64_t *>(lwe_array_in),
+           static_cast<const uint64_t *>(lwe_input_indexes),
+           static_cast<const uint64_t *>(ksk), lwe_dimension_in, out_len,
+           body_pos, base_log, level_count, num_samples);
     t_last_ks_kernel = "ks_f64";
     return;
   }
   // the s32-digit MAC holds digits up to base_log 31; wider digits (|d| up to
   // 2^(base_log - 1), l = 1) take the s64 instance
   const bool wide_digits = base_log >= 32;
-  (wide_digits ? keyswitch_kernel<int64_t> : keyswitch_kernel<int32_t>)
-      <<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<uint64_t *>(lwe_array_out),
-      static_cast<const uint64_t *>(lwe_output_indexes),
-      static_cast<const uint64_t *>(lwe_array_in),
-      static_cast<const uint64_t *>(lwe_input_indexes),
-      static_cast<const uint64_t *>(ksk), lwe_dimension_in, out_len, body_pos,
-      base_log, level_count, num_samples);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(wide_digits ? keyswitch_kernel<int64_t> : keyswitch_kernel<int32_t>,
+         {grid, 256, 0, st, gpu_index}, static_cast<uint64_t *>(lwe_array_out),
+         static_cast<const uint64_t *>(lwe_output_indexes),
+         static_cast<const uint64_t *>(lwe_array_in),
+         static_cast<const uint64_t *>(lwe_input_indexes),
+         static_cast<const uint64_t *>(ksk), lwe_dimension_in, out_len,
+         body_pos, base_log, level_count, num_samples);
   t_last_ks_kernel = wide_digits ? "ks_int_wide" : "ks_int";
 }
 
@@ -1747,15 +1591,14 @@ void cuda_keyswitch_lwe_ciphertext_vector_64_32_async(
                       "level_count %u)", base_log, level_count);
   dim3 grid((num_samples + KS_TS - 1) / KS_TS,
             (lwe_dimension_out + 1 + KS_TO - 1) / KS_TO);
-  keyswitch_64_32_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<uint32_t *>(lwe_array_out),
-      static_cast<const uint64_t *>(lwe_output_indexes),
-      static_cast<const uint64_t *>(lwe_array_in),
-      static_cast<const uint64_t *>(lwe_input_indexes),
-      static_cast<const uint32_t *>(ksk), lwe_dimension_in, lwe_dimension_out,
-      base_log, level_count, num_samples);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(keyswitch_64_32_kernel,
+         {grid, 256, 0, static_cast<cudaStream_t>(stream), gpu_index},
+         static_cast<uint32_t *>(lwe_array_out),
+         static_cast<const uint64_t *>(lwe_output_indexes),
+         static_cast<const uint64_t *>(lwe_array_in),
+         static_cast<const uint64_t *>(lwe_input_indexes),
+         static_cast<const uint32_t *>(ksk), lwe_dimension_in,
+         lwe_dimension_out, base_log, level_count, num_samples);
   t_last_ks_kernel = "ks_64_32";
 }
 
@@ -1788,14 +1631,12 @@ void cuda_glwe_sample_extract_64_async(
                           num_lwes_stored_per_glwe >= 1 &&
                           num_lwes_stored_per_glwe <= polynomial_size,
                       "Cuda error (sample extract): invalid extraction counts");
-  glwe_sample_extract_kernel<<<num_nths, 256, 0,
-                               static_cast<cudaStream_t>(stream)>>>(
-      static_cast<uint64_t *>(lwe_array_out),
-      static_cast<const uint64_t *>(glwe_array_in), nth_array,
-      num_lwes_to_extract_per_glwe, num_lwes_stored_per_glwe, glwe_dimension,
-      polynomial_size);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(glwe_sample_extract_kernel,
+         {num_nths, 256, 0, static_cast<cudaStream_t>(stream), gpu_index},
+         static_cast<uint64_t *>(lwe_array_out),
+         static_cast<const uint64_t *>(glwe_array_in), nth_array,
+         num_lwes_to_extract_per_glwe, num_lwes_stored_per_glwe,
+         glwe_dimension, polynomial_size);
 }
 
 void cuda_modulus_switch_64_async(void *stream, uint32_t gpu_index,
@@ -1807,12 +1648,11 @@ void cuda_modulus_switch_64_async(void *stream, uint32_t gpu_index,
   B200_PANIC_IF_FALSE(log_modulus >= 1 && log_modulus <= 63,
                       "Cuda error (modulus switch): log_modulus %u out of range",
                       log_modulus);
-  modulus_switch_kernel<<<(size + 255) / 256, 256, 0,
-                          static_cast<cudaStream_t>(stream)>>>(
-      static_cast<uint64_t *>(lwe_out), static_cast<const uint64_t *>(lwe_in),
-      size, log_modulus);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(modulus_switch_kernel,
+         {(size + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream),
+          gpu_index},
+         static_cast<uint64_t *>(lwe_out),
+         static_cast<const uint64_t *>(lwe_in), size, log_modulus);
 }
 
 void cuda_modulus_switch_inplace_64_async(void *stream, uint32_t gpu_index,
@@ -1830,12 +1670,10 @@ void cuda_centered_modulus_switch_64_async(void *stream, uint32_t gpu_index,
   B200_PANIC_IF_FALSE(log_modulus >= 1 && log_modulus <= 63,
                       "Cuda error (modulus switch): log_modulus %u out of range",
                       log_modulus);
-  centered_modulus_switch_kernel<<<1, 256, 0,
-                                   static_cast<cudaStream_t>(stream)>>>(
-      static_cast<uint64_t *>(lwe_out), static_cast<const uint64_t *>(lwe_in),
-      lwe_dimension, log_modulus);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(centered_modulus_switch_kernel,
+         {1, 256, 0, static_cast<cudaStream_t>(stream), gpu_index},
+         static_cast<uint64_t *>(lwe_out),
+         static_cast<const uint64_t *>(lwe_in), lwe_dimension, log_modulus);
 }
 
 // ===========================================================================
@@ -1849,12 +1687,11 @@ void b200_forward_negacyclic_fft_async(void *stream, uint32_t gpu_index,
   B200_PANIC_IF_FALSE(polynomial_size == 2048,
                       "b200_forward_negacyclic_fft_async: N must be 2048");
   const DeviceTables &t = device_tables(gpu_index, 0);
-  forward_fft_natural_kernel<<<total_polynomials, 64, 0,
-                               static_cast<cudaStream_t>(stream)>>>(
-      static_cast<cplx *>(output), static_cast<const cplx *>(input),
-      t.fft1024);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(forward_fft_natural_kernel,
+         {total_polynomials, 64, 0, static_cast<cudaStream_t>(stream),
+          gpu_index},
+         static_cast<cplx *>(output), static_cast<const cplx *>(input),
+         t.fft1024);
 }
 
 void b200_oprf_expand_seeded_lwe_64_async(
@@ -1877,14 +1714,8 @@ void b200_grouped_oprf_64_async(
   set_device(gpu_index);
   check_polynomial_size(polynomial_size);
   const bool multi_bit = grouping_factor > 1;
-  const PbsScratch *s = reinterpret_cast<const PbsScratch *>(buffer);
-  B200_PANIC_IF_FALSE(s && s->magic == SCRATCH_MAGIC &&
-                          s->type == (multi_bit ? MULTI_BIT : CLASSICAL),
-                      "Cuda error (OPRF): invalid scratch buffer");
-  B200_PANIC_IF_FALSE(
-      s->glwe_dim == glwe_dimension && s->poly_size == polynomial_size &&
-          s->level_count == level_count,
-      "Cuda error (OPRF): scratch buffer was created for other parameters");
+  pbs_scratch(buffer, multi_bit ? MULTI_BIT : CLASSICAL, "OPRF",
+              PbsShape{glwe_dimension, polynomial_size, level_count});
   if (num_blocks == 0)
     return;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1894,9 +1725,8 @@ void b200_grouped_oprf_64_async(
       &ws, (in_words + num_blocks) * sizeof(uint64_t),
       workspace_pool(gpu_index), st));
   uint64_t *idx = ws + in_words;
-  oprf_iota_kernel<<<(num_blocks + 255) / 256, 256, 0, st>>>(idx, num_blocks);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(oprf_iota_kernel, {(num_blocks + 255) / 256, 256, 0, st, gpu_index},
+         idx, num_blocks);
   oprf_expand(st, gpu_index, ws, aes_key, counter_lo, counter_hi, 0,
               lwe_dimension, num_blocks, ilog2_exact(polynomial_size) + 1);
   // centered_ms = 0 whatever the scratch object says: the switched values
@@ -1908,11 +1738,10 @@ void b200_grouped_oprf_64_async(
              base_log, level_count, multi_bit ? grouping_factor : 1, num_blocks,
              1, 0, 0);
   const uint64_t big_n = (uint64_t)glwe_dimension * polynomial_size;
-  oprf_add_corrections_kernel<<<(num_blocks + 255) / 256, 256, 0, st>>>(
-      static_cast<uint64_t *>(lwe_out),
-      static_cast<const uint64_t *>(corrections), big_n, num_blocks);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(oprf_add_corrections_kernel,
+         {(num_blocks + 255) / 256, 256, 0, st, gpu_index},
+         static_cast<uint64_t *>(lwe_out),
+         static_cast<const uint64_t *>(corrections), big_n, num_blocks);
   B200_CHECK(cudaFreeAsync(ws, st));
 }
 
@@ -1942,23 +1771,15 @@ void b200_expand_without_verification_64_async(
   set_device(gpu_index);
   check_polynomial_size(polynomial_size);
   const bool multi_bit = grouping_factor > 1;
-  const PbsScratch *s = reinterpret_cast<const PbsScratch *>(buffer);
-  B200_PANIC_IF_FALSE(s && s->magic == SCRATCH_MAGIC &&
-                          s->type == (multi_bit ? MULTI_BIT : CLASSICAL),
-                      "Cuda error (expand): invalid scratch buffer");
-  B200_PANIC_IF_FALSE(
-      s->glwe_dim == glwe_dimension && s->poly_size == polynomial_size &&
-          s->level_count == pbs_level_count,
-      "Cuda error (expand): scratch buffer was created for other parameters");
-  B200_PANIC_IF_FALSE(casting_ksk && (!casting_to_big || computing_ksk),
-                      "Cuda error (expand): missing keyswitching key");
   const uint64_t T = compact_lists_total(num_lwes_per_compact_list,
                                          num_compact_lists,
                                          compact_lwe_dimension);
-  B200_PANIC_IF_FALSE(2 * T <= s->max_samples,
-                      "Cuda error (expand): scratch buffer made for %u "
-                      "samples, the call unpacks %llu", s->max_samples,
-                      (unsigned long long)(2 * T));
+  const PbsScratch &s =
+      pbs_scratch(buffer, multi_bit ? MULTI_BIT : CLASSICAL, "expand",
+                  PbsShape{glwe_dimension, polynomial_size, pbs_level_count},
+                  2 * T);
+  B200_PANIC_IF_FALSE(casting_ksk && (!casting_to_big || computing_ksk),
+                      "Cuda error (expand): missing keyswitching key");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const uint64_t big_n = (uint64_t)glwe_dimension * polynomial_size;
   const uint64_t exp_words = T * (compact_lwe_dimension + 1);
@@ -1992,16 +1813,15 @@ void b200_expand_without_verification_64_async(
         casting_level_count, (uint32_t)T);
   }
   const uint32_t samples = (uint32_t)(2 * T);
-  compact_unpack_index_kernel<<<(samples + 255) / 256, 256, 0, st>>>(
-      in_idx, out_idx, samples);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(compact_unpack_index_kernel,
+         {(samples + 255) / 256, 256, 0, st, gpu_index}, in_idx, out_idx,
+         samples);
   launch_pbs(st, gpu_index, static_cast<uint64_t *>(lwe_array_out), out_idx,
              static_cast<const uint64_t *>(lut_vector),
              static_cast<const uint64_t *>(lut_indexes), small, in_idx,
              bootstrapping_key, lwe_dimension, glwe_dimension, polynomial_size,
              pbs_base_log, pbs_level_count, multi_bit ? grouping_factor : 1,
-             samples, 1, 0, s->centered_ms);
+             samples, 1, 0, s.centered_ms);
   B200_CHECK(cudaFreeAsync(ws, st));
 }
 
@@ -2054,10 +1874,8 @@ void b200_rerand_64_async(void *stream, uint32_t gpu_index, void *lwe_array,
         (uint32_t)T);
   }
   const uint64_t blocks = std::min<uint64_t>((out_words + 255) / 256, 65535u);
-  rerand_add_kernel<<<(unsigned)blocks, 256, 0, st>>>(
-      static_cast<uint64_t *>(lwe_array), zeros, out_words);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(rerand_add_kernel, {(unsigned)blocks, 256, 0, st, gpu_index},
+         static_cast<uint64_t *>(lwe_array), zeros, out_words);
   B200_CHECK(cudaFreeAsync(ws, st));
 }
 
@@ -2102,11 +1920,10 @@ void cuda_packing_keyswitch_lwe_list_to_glwe_64_async(
   keyswitch_64(stream, gpu_index, rows, nullptr, lwe_array_in, nullptr,
                fp_ksk_array, input_lwe_dimension, (k + 1) * N, k * N, base_log,
                level_count, num_lwes);
-  pack_glwe_kernel<<<dim3((k + 1) * N / PACK_THREADS, 1), PACK_THREADS, 0,
-                     st>>>(static_cast<uint64_t *>(glwe_array_out), rows, k, N,
-                           num_lwes, num_lwes, 0);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(pack_glwe_kernel,
+         {dim3((k + 1) * N / PACK_THREADS, 1), PACK_THREADS, 0, st, gpu_index},
+         static_cast<uint64_t *>(glwe_array_out), rows, k, N, num_lwes,
+         num_lwes, 0);
 }
 
 void cleanup_cuda_packing_keyswitch_lwe_list_to_glwe_64(
@@ -2153,18 +1970,16 @@ void b200_compress_lwe_ciphertexts_64_async(
                                      workspace_pool(gpu_index), st));
   uint64_t *scaled = ws, *rows = ws + in_words;
   const uint64_t blocks = std::min<uint64_t>((in_words + 255) / 256, 65535u);
-  compression_scale_kernel<<<(unsigned)blocks, 256, 0, st>>>(
-      scaled, static_cast<const uint64_t *>(lwe_array_in), in_words, scale);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(compression_scale_kernel, {(unsigned)blocks, 256, 0, st, gpu_index},
+         scaled, static_cast<const uint64_t *>(lwe_array_in), in_words, scale);
   keyswitch_64(stream, gpu_index, rows, nullptr, scaled, nullptr, packing_ksk,
                lwe_dimension, (k + 1) * N, k * N, base_log, level_count,
                num_lwes);
-  pack_glwe_kernel<<<dim3((k + 1) * N / PACK_THREADS, num_glwes), PACK_THREADS,
-                     0, st>>>(static_cast<uint64_t *>(packed_out), rows, k, N,
-                              num_lwes, lwe_per_glwe, storage_log_modulus);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(pack_glwe_kernel,
+         {dim3((k + 1) * N / PACK_THREADS, num_glwes), PACK_THREADS, 0, st,
+          gpu_index},
+         static_cast<uint64_t *>(packed_out), rows, k, N, num_lwes,
+         lwe_per_glwe, storage_log_modulus);
   B200_CHECK(cudaFreeAsync(ws, st));
 }
 
@@ -2181,19 +1996,9 @@ void b200_decompress_lwe_ciphertexts_64_async(
                            storage_log_modulus);
   check_polynomial_size(polynomial_size);
   const bool multi_bit = grouping_factor > 1;
-  const PbsScratch *s = reinterpret_cast<const PbsScratch *>(buffer);
-  B200_PANIC_IF_FALSE(s && s->magic == SCRATCH_MAGIC &&
-                          s->type == (multi_bit ? MULTI_BIT : CLASSICAL),
-                      "Cuda error (decompression): invalid scratch buffer");
-  B200_PANIC_IF_FALSE(
-      s->glwe_dim == glwe_dimension && s->poly_size == polynomial_size &&
-          s->level_count == level_count,
-      "Cuda error (decompression): scratch buffer was created for other "
-      "parameters");
-  B200_PANIC_IF_FALSE(num_indexes <= s->max_samples,
-                      "Cuda error (decompression): scratch buffer made for %u "
-                      "samples, the call decompresses %u", s->max_samples,
-                      num_indexes);
+  pbs_scratch(buffer, multi_bit ? MULTI_BIT : CLASSICAL, "decompression",
+              PbsShape{glwe_dimension, polynomial_size, level_count},
+              num_indexes);
   if (num_indexes == 0)
     return;
   // trivial PBS indexes, one all-zero LUT index per sample, then the list
@@ -2218,14 +2023,12 @@ void b200_decompress_lwe_ciphertexts_64_async(
   uint64_t *lut_idx = iota + num_indexes, *list_idx = lut_idx + num_indexes;
   B200_CHECK(cudaMemcpyAsync(iota, h_idx.data(), h_idx.size() * sizeof(uint64_t),
                              cudaMemcpyHostToDevice, st));
-  unpack_extract_kernel<<<dim3((big_n + 1 + 255) / 256,
-                               std::min<uint32_t>(num_indexes, 65535u)),
-                          256, 0, st>>>(
-      extracted, static_cast<const uint64_t *>(packed_in), list_idx, num_indexes,
-      compression_glwe_dimension, compression_polynomial_size, lwe_per_glwe,
-      storage_log_modulus);
-  B200_CHECK(cudaGetLastError());
-  count_launch();
+  launch(unpack_extract_kernel,
+         {dim3((big_n + 1 + 255) / 256, std::min<uint32_t>(num_indexes, 65535u)),
+          256, 0, st, gpu_index},
+         extracted, static_cast<const uint64_t *>(packed_in), list_idx,
+         num_indexes, compression_glwe_dimension, compression_polynomial_size,
+         lwe_per_glwe, storage_log_modulus);
   // no centered-mean correction: the extracted words are exact multiples of
   // 2^(64 - storage_log_modulus) and must not move (as in the grouped OPRF)
   launch_pbs(st, gpu_index, static_cast<uint64_t *>(lwe_out), iota,

@@ -59,6 +59,5 @@ struct DeviceTables {
 const DeviceTables &device_tables(uint32_t gpu_index, uint32_t logM);
 
 void set_device(uint32_t gpu_index);
-void count_launch();
 
 } // namespace b200
