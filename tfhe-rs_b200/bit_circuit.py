@@ -6,7 +6,8 @@ ciphertext the engine bootstraps is a *linear step*
     sum_i c_i * w_i + c_0
 
 over wires w_i that are fresh client bits or PBS outputs, followed by one
-keyswitch and one PBS with a LUT of the fixed set `lut_functions()`.  The compiler keeps
+keyswitch and one PBS with a LUT of the fixed set `lut_functions()` (or of the
+circuit's own tables, `Circuit.add_lut`, indexed after it).  The compiler keeps
 every such input inside the noise contract of the 2_2 parameter sets
 (tfhe-rs `MaxNoiseLevel` 5, scalar multiplication multiplying the noise level):
 
@@ -70,15 +71,19 @@ def lut_functions() -> List[List[int]]:
 
 # largest value each LUT can output (the value range of the wire it makes)
 LUT_VMAX = [1] * 9 + [2, 1]
+NUM_FIXED_LUTS = len(LUT_VMAX)
+MAX_BLOCK_VALUE = 3   # message modulus - 1: the largest value an output block may hold
 
 
-def lut_glwes(polynomial_size: int, glwe_dimension: int) -> np.ndarray:
-    """The accumulators of `lut_functions()` for the 2_2 encoding."""
+def lut_glwes(polynomial_size: int, glwe_dimension: int, tables: Optional[Sequence[Sequence[int]]] = None
+              ) -> np.ndarray:
+    """The accumulators of `tables` (default `lut_functions()`) for the 2_2 encoding."""
     from . import algorithms
 
     delta = (1 << 63) // TOTAL_MOD
     return np.stack([algorithms.generate_programmable_bootstrap_glwe_lut(
-        polynomial_size, glwe_dimension + 1, TOTAL_MOD, delta, f) for f in lut_functions()])
+        polynomial_size, glwe_dimension + 1, TOTAL_MOD, delta, f)
+        for f in (lut_functions() if tables is None else tables)])
 
 
 # ---------------------------------------------------------------------------
@@ -95,7 +100,12 @@ class Circuit:
     `lut` terms read the wire's *value* (a bit, or a carry state in {0, 1, 2});
     a term on an XOR form of several wires is stored first.  Only `lut` gates
     may read a wire whose values exceed 1 (a carry state): the bit gates and
-    the outputs raise ValueError on one."""
+    `output` raise ValueError on one.  `output_blocks` is the explicit opt-in
+    for outputs that are 2_2 message blocks (values up to MAX_BLOCK_VALUE).
+
+    A circuit may carry LUT tables of its own (`add_lut`): they take the
+    indexes after the fixed set, and the executors upload their accumulators
+    with it."""
 
     def __init__(self, name: str):
         self.name = name
@@ -105,6 +115,7 @@ class Circuit:
         self.num_iconsts = 0
         self.outputs: List[int] = []
         self.vmax: List[int] = []   # largest value of each wire
+        self.extra_luts: List[Tuple[int, ...]] = []   # circuit-local tables, LUT index NUM_FIXED_LUTS + i
 
     def _add(self, g, vmax: int = 1) -> int:
         self.gates.append(g)
@@ -155,8 +166,26 @@ class Circuit:
         self._bits(a, b)
         return self._add(("and", a, b))
 
+    def add_lut(self, table: Sequence[int]) -> int:
+        """A LUT of this circuit: f over the 16 values of the padded message
+        space, outputs in [0, MAX_VALUE]; returns its LUT index."""
+        table = tuple(int(v) for v in table)
+        if len(table) != TOTAL_MOD or min(table) < 0 or max(table) > MAX_VALUE:
+            raise ValueError(f"{self.name}: a LUT maps the {TOTAL_MOD} values to [0, {MAX_VALUE}]")
+        self.extra_luts.append(table)
+        return NUM_FIXED_LUTS + len(self.extra_luts) - 1
+
+    def lut_tables(self) -> List[List[int]]:
+        """every table a `lut` gate of this circuit may name, by LUT index"""
+        return lut_functions() + [list(t) for t in self.extra_luts]
+
+    def lut_vmax(self, lut: int) -> int:
+        return LUT_VMAX[lut] if lut < NUM_FIXED_LUTS else max(self.extra_luts[lut - NUM_FIXED_LUTS])
+
     def lut(self, terms: Sequence[Tuple[int, int]], c0: int, lut: int) -> int:
-        return self._add(("lut", tuple((int(w), int(c)) for w, c in terms), int(c0), int(lut)), LUT_VMAX[lut])
+        if not 0 <= lut < NUM_FIXED_LUTS + len(self.extra_luts):
+            raise ValueError(f"{self.name}: unknown LUT {lut}")
+        return self._add(("lut", tuple((int(w), int(c)) for w, c in terms), int(c0), int(lut)), self.lut_vmax(lut))
 
     def mat(self, a: int) -> int:
         self._bits(a)
@@ -166,9 +195,18 @@ class Circuit:
         self._bits(*ws)
         self.outputs.extend(ws)
 
+    def output_blocks(self, ws: Sequence[int]):
+        """Outputs that are message blocks: wires holding values up to
+        MAX_BLOCK_VALUE (a LUT wire packing two bits, or a bit)."""
+        for w in ws:
+            if self.vmax[w] > MAX_BLOCK_VALUE:
+                raise ValueError(f"{self.name}: wire {w} holds values up to {self.vmax[w]}, more than a "
+                                 f"block's {MAX_BLOCK_VALUE}")
+        self.outputs.extend(ws)
+
     def evaluate(self, shared_bits, instance_bits, iconst_bits) -> List[int]:
         """Direct evaluation of one instance (the reference semantics)."""
-        luts = lut_functions()
+        luts = self.lut_tables()
         val: List[int] = []
         for g in self.gates:
             op = g[0]
@@ -244,6 +282,11 @@ class Schedule:
     num_iconsts: int
     pbs_per_instance_rows: int = 0
     pbs_shared_rows: int = 0
+    extra_luts: Tuple[Tuple[int, ...], ...] = ()   # the circuit's own tables, after lut_functions()
+
+    def lut_tables(self) -> List[List[int]]:
+        """the f tables of the LUT indexes in row_lut"""
+        return lut_functions() + [list(t) for t in self.extra_luts]
 
     @property
     def num_layers(self) -> int:
@@ -350,7 +393,7 @@ class _Compiler:
         assert noise <= MAX_NOISE_LEVEL and 0 <= lo and hi <= MAX_VALUE, (terms, body, iterms, lut)
         layer = 1 + max([self.atoms[a].ready for a, _ in terms], default=0)
         shared = all(self.atoms[a].shared for a, _ in terms) and not iterms
-        out = self.new_atom(layer, LUT_VMAX[lut], shared)
+        out = self.new_atom(layer, self.circ.lut_vmax(lut), shared)
         self.rows.append(Row(terms, body, iterms, lut, out, layer, shared))
         self.memo[key] = out
         return out
@@ -547,7 +590,8 @@ def compile_circuit(circuit: Circuit, num_instances: int = 1) -> Schedule:
         instance_input_slots=np.array([gslot(comp.input_atoms[(False, i)])
                                        for i in range(circuit.num_instance_inputs)], dtype=np.int64),
         output_slots=np.array([gslot(a) for a in outs], dtype=np.int64), num_iconsts=circuit.num_iconsts,
-        pbs_per_instance_rows=sum(not r.shared for r in ordered), pbs_shared_rows=sum(r.shared for r in ordered))
+        pbs_per_instance_rows=sum(not r.shared for r in ordered), pbs_shared_rows=sum(r.shared for r in ordered),
+        extra_luts=tuple(circuit.extra_luts))
 
 
 # one compiled schedule per live circuit object, whatever the instance counts
@@ -585,7 +629,7 @@ def run_cleartext(sched: Schedule, shared_bits, instance_bits=None, iconst_bits=
                               sched.addr(sched.instance_input_slots[None, :], np.arange(I)[:, None]).reshape(-1)])
     lvl[written] = 1
     body = sched.body(iconst_bits) if sched.num_iconsts else np.repeat(sched.body_base[:, None], I, axis=1)
-    luts = np.array(lut_functions(), dtype=np.int64)
+    luts = np.array(sched.lut_tables(), dtype=np.int64)
 
     def poison(slots):
         if len(slots):

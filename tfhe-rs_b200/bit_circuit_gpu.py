@@ -40,7 +40,8 @@ def body_words(sched: bc.Schedule, iconst_bits: Optional[np.ndarray]) -> np.ndar
 
 
 class _DeviceSchedule:
-    def __init__(self, sched: bc.Schedule, device, stream):
+    def __init__(self, sched: bc.Schedule, device, stream, luts: gpu.CudaGlweCiphertextList):
+        self.luts = luts  # accumulators of sched.lut_tables()
         luts, dests = sched.gpu_tables()
         widest = max([sched.layer_outputs(L) for L in range(sched.num_layers)], default=0)
         with torch.cuda.stream(stream):
@@ -119,12 +120,20 @@ class CudaBitCircuitRunner:
     def device_tables(self, circuit: bc.Circuit, sched: bc.Schedule) -> _DeviceSchedule:
         """The schedule's device tables, uploaded on first use; the least
         recently used pair beyond MAX_TABLES is dropped (its tensors were
-        allocated on the work stream, so queued work that reads them is safe)."""
+        allocated on the work stream, so queued work that reads them is safe).
+        A circuit with LUTs of its own gets its own accumulators (the fixed
+        set, then its tables); the others share the runner's."""
         key = (circuit, sched.num_instances)
         if key in self._tables:
             self._tables.move_to_end(key)
         else:
-            self._tables[key] = _DeviceSchedule(sched, self.device, self.streams.streams[0])
+            luts = self.luts
+            if sched.extra_luts:
+                bsk = self.skey.bsk
+                luts = gpu.CudaGlweCiphertextList.from_glwe_ciphertext_list(
+                    bc.lut_glwes(bsk.polynomial_size, bsk.glwe_dimension, sched.lut_tables()), bsk.glwe_dimension,
+                    bsk.polynomial_size, self.streams)
+            self._tables[key] = _DeviceSchedule(sched, self.device, self.streams.streams[0], luts)
             while len(self._tables) > self.MAX_TABLES:
                 self._tables.popitem(last=False)
         return self._tables[key]
@@ -217,7 +226,7 @@ class CudaBitCircuitRunner:
             T.layer_shared_rows.ctypes.data_as(C.POINTER(C.c_uint32)),
             T.row_offsets.data_ptr(), T.term_slots.data_ptr(), T.term_coefs.data_ptr(), body.data_ptr(),
             T.lut_idx.data_ptr(), T.out_idx.data_ptr(), T.in_idx.data_ptr(), ksk.d_vec.as_c_ptr(),
-            ksk.decomp_base_log, ksk.decomp_level_count, self.luts.d_vec.as_c_ptr(), bsk.d_vec.as_c_ptr(),
+            ksk.decomp_base_log, ksk.decomp_level_count, T.luts.d_vec.as_c_ptr(), bsk.d_vec.as_c_ptr(),
             scratch.buf, big, bsk.input_lwe_dimension, bsk.glwe_dimension, bsk.polynomial_size,
             bsk.decomp_base_log, bsk.decomp_level_count, bsk.grouping_factor if skey.multi_bit else 1)
         with torch.cuda.stream(st):
