@@ -91,7 +91,8 @@ def lut_glwes(polynomial_size: int, glwe_dimension: int, tables: Optional[Sequen
 # ---------------------------------------------------------------------------
 class Circuit:
     """A DAG of gates on wire ids.  Gates:
-      ('in', shared, index)        fresh client bit (shared or per instance)
+      ('in', shared, index)        fresh client bit (shared or per instance),
+                                   or message block (`input_block`, vmax 3)
       ('const', b)                 shared constant bit
       ('iconst', index)            per-instance plaintext bit (given per call)
       ('xor', a, b), ('not', a), ('and', a, b)
@@ -99,9 +100,10 @@ class Circuit:
       ('mat', a)                   store `a` as a PBS output (a refresh point)
     `lut` terms read the wire's *value* (a bit, or a carry state in {0, 1, 2});
     a term on an XOR form of several wires is stored first.  Only `lut` gates
-    may read a wire whose values exceed 1 (a carry state): the bit gates and
-    `output` raise ValueError on one.  `output_blocks` is the explicit opt-in
-    for outputs that are 2_2 message blocks (values up to MAX_BLOCK_VALUE).
+    may read a wire whose values exceed 1 (a carry state, or a client message
+    block made by `input_block`): the bit gates and `output` raise
+    ValueError on one.  `output_blocks` is the explicit opt-in for outputs
+    that are 2_2 message blocks (values up to MAX_BLOCK_VALUE).
 
     A circuit may carry LUT tables of its own (`add_lut`): they take the
     indexes after the fixed set, and the executors upload their accumulators
@@ -137,6 +139,16 @@ class Circuit:
 
     def inputs(self, count: int, shared: bool) -> List[int]:
         return [self.input(shared) for _ in range(count)]
+
+    def input_block(self, shared: bool) -> int:
+        """A fresh client message block (values up to MAX_BLOCK_VALUE): only
+        `lut` gates may read it, like a carry state."""
+        w = self.input(shared)
+        self.vmax[w] = MAX_BLOCK_VALUE
+        return w
+
+    def inputs_block(self, count: int, shared: bool) -> List[int]:
+        return [self.input_block(shared) for _ in range(count)]
 
     def const(self, b: int) -> int:
         return self._add(("const", int(b) & 1))
@@ -197,12 +209,20 @@ class Circuit:
 
     def output_blocks(self, ws: Sequence[int]):
         """Outputs that are message blocks: wires holding values up to
-        MAX_BLOCK_VALUE (a LUT wire packing two bits, or a bit)."""
+        MAX_BLOCK_VALUE (a LUT wire packing two bits, or a bit).  A block
+        input passed straight through is refreshed by a PBS on a circuit-local
+        identity table (the parity refresh of bit inputs would keep x mod 2)."""
         for w in ws:
             if self.vmax[w] > MAX_BLOCK_VALUE:
                 raise ValueError(f"{self.name}: wire {w} holds values up to {self.vmax[w]}, more than a "
                                  f"block's {MAX_BLOCK_VALUE}")
-        self.outputs.extend(ws)
+        ident = tuple(x if x <= MAX_BLOCK_VALUE else 0 for x in range(TOTAL_MOD))
+        for w in ws:
+            if self.gates[w][0] == "in" and self.vmax[w] > 1:
+                lut = (NUM_FIXED_LUTS + self.extra_luts.index(ident) if ident in self.extra_luts
+                       else self.add_lut(ident))
+                w = self.lut([(w, 1)], 0, lut)
+            self.outputs.append(w)
 
     def evaluate(self, shared_bits, instance_bits, iconst_bits) -> List[int]:
         """Direct evaluation of one instance (the reference semantics)."""
@@ -470,10 +490,10 @@ class _Compiler:
 
     def run(self):
         forms: List[_Form] = []
-        for g in self.circ.gates:
+        for gi, g in enumerate(self.circ.gates):
             op = g[0]
             if op == "in":
-                a = self.new_atom(0, 1, g[1])
+                a = self.new_atom(0, self.circ.vmax[gi], g[1])   # 1, or MAX_BLOCK_VALUE for a block input
                 self.input_atoms[(g[1], g[2])] = a
                 f = _Form({a})
             elif op == "const":
@@ -498,6 +518,9 @@ class _Compiler:
             f = forms[w]
             if len(f.atoms) == 1 and f.c == 0 and not f.k:
                 a = next(iter(f.atoms))
+                if a in inputs and self.atoms[a].vmax > 1:
+                    # `output_blocks` refreshes block inputs itself; parity would keep x mod 2
+                    raise ValueError(f"{self.circ.name}: a block input is output without a refresh")
                 # a client bit passed through is refreshed by a PBS of its own
                 outs.append(self.emit([(a, 1)], 0, [], LUT_PARITY) if a in inputs else a)
             else:

@@ -290,19 +290,49 @@ class CudaBlockEngine(BlockEngine):
 
 
 class CudaUnsignedRadixCiphertext:
-    """integer/gpu/ciphertext: a vector of shortint blocks on one GPU."""
+    """integer/gpu/ciphertext: a vector of shortint blocks on one GPU, least
+    significant first.  It may hold `num_inputs` integers of `num_blocks`
+    blocks each, instance-major: `blocks` is [num_inputs * num_blocks,
+    big + 1]; the radix operations run them as instances of one schedule."""
+    signed = False
 
-    def __init__(self, blocks):
+    def __init__(self, blocks, num_inputs: int = 1):
         self.blocks = blocks
+        self.num_inputs = num_inputs
 
     @property
     def num_blocks(self):
-        return self.blocks.shape[0]
+        return self.blocks.shape[0] // self.num_inputs
+
+
+class CudaSignedRadixCiphertext(CudaUnsignedRadixCiphertext):
+    """A two's-complement radix integer: the sign is bit 1 of the top block."""
+    signed = True
+
+
+class CudaBooleanBlock:
+    """One block holding 0 or 1 per input: `blocks` is [num_inputs, big + 1]."""
+
+    def __init__(self, blocks, num_inputs: int = 1):
+        self.blocks = blocks
+        self.num_inputs = num_inputs
 
 
 class CudaRadixServerKey:
-    """Mirror of integer::gpu::CudaServerKey for the multiplication path
-    (integer/gpu/server_key/radix/mul.rs:167)."""
+    """Mirror of integer::gpu::CudaServerKey: the multiplication path
+    (integer/gpu/server_key/radix/mul.rs:167), and comparisons, selects,
+    additions, subtractions, bitwise operations and erc7984's transfer,
+    compiled to KS -> PBS layers (`radix`) and run by a bit-circuit runner of
+    its own (created on first use) with `b200_bit_circuit_64_async`.
+
+    Those operations take ciphertexts of one kind (unsigned or signed), one
+    block count and one `num_inputs`, on 2_2 keys, and raise ValueError before
+    any GPU work otherwise.  The work runs on the server key's first stream
+    after the caller's current stream; inputs may be dropped as soon as a
+    call returns, and the caller's stream waits for the result (see
+    `bit_circuit_gpu`)."""
+
+    _runner = None
 
     def __init__(self, server_key, lut_glwe_list_np=None, glwe_dimension=1, polynomial_size=2048):
         if lut_glwe_list_np is None:  # the 7 accumulators of lut_functions(), 2+2-bit blocks, one padding bit
@@ -316,3 +346,182 @@ class CudaRadixServerKey:
 
     def unchecked_mul(self, lhs: CudaUnsignedRadixCiphertext, rhs: CudaUnsignedRadixCiphertext):
         return CudaUnsignedRadixCiphertext(unchecked_mul(self.engine, lhs.blocks, rhs.blocks))
+
+    # -- compiled radix circuits ------------------------------------------------
+    @property
+    def runner(self):
+        """The bit-circuit runner of the radix circuits, created on first use
+        (its device tables are its own: AES or Trivium runners keep theirs)."""
+        if self._runner is None:
+            skey = self.engine.skey
+            moduli = (getattr(skey, "message_modulus", None), getattr(skey, "carry_modulus", None))
+            if moduli != (MSG_MOD, TOTAL_MOD // MSG_MOD):
+                raise ValueError(f"radix circuits need a 2_2 server key, got message / carry moduli {moduli}")
+            from . import bit_circuit_gpu
+
+            self._runner = bit_circuit_gpu.CudaBitCircuitRunner(skey)
+        return self._runner
+
+    @staticmethod
+    def _operands(*cts):
+        """(ciphertext type, num_blocks, num_inputs) shared by all operands"""
+        from . import radix
+
+        first = cts[0]
+        for ct in cts:
+            if not isinstance(ct, CudaUnsignedRadixCiphertext):
+                raise ValueError(f"expected a radix ciphertext, got {type(ct).__name__}")
+            if type(ct) is not type(first):
+                raise ValueError(f"operands differ in signedness: {type(first).__name__} and {type(ct).__name__}")
+            I = ct.num_inputs
+            if isinstance(I, bool) or not isinstance(I, (int, np.integer)) or I < 1 or ct.blocks.shape[0] % I:
+                raise ValueError(f"{ct.blocks.shape[0]} blocks do not hold num_inputs = {I!r} integers")
+            if I != first.num_inputs:
+                raise ValueError(f"operands differ in num_inputs: {first.num_inputs} and {I}")
+            if ct.num_blocks != first.num_blocks:
+                raise ValueError(f"operands differ in block count: {first.num_blocks} and {ct.num_blocks}")
+        return type(first), radix.check_num_blocks(first.num_blocks), int(first.num_inputs)
+
+    def _run(self, op, signed, n, I, blocks, iconsts=None):
+        """the circuit of (op, n, signed) on the operands' blocks, concatenated
+        per instance; returns the outputs [I, outputs, big + 1]"""
+        import torch
+
+        from . import radix
+
+        W = blocks[0].shape[1]
+        parts = [b.reshape(I, -1, W) for b in blocks]
+        inst = parts[0] if len(parts) == 1 else torch.cat(parts, 1)
+        return self.runner.run(radix.circuit(op, n, signed), None, inst.reshape(-1, W), iconsts, I).view(I, -1, W)
+
+    @staticmethod
+    def _radix(kind, out, I):
+        return kind(out.reshape(-1, out.shape[-1]), I)
+
+    def _binary(self, op, lhs, rhs):
+        kind, n, I = self._operands(lhs, rhs)
+        return kind, I, self._run(op, kind.signed, n, I, [lhs.blocks, rhs.blocks])
+
+    def _compare(self, op, lhs, rhs) -> CudaBooleanBlock:
+        _, I, out = self._binary(op, lhs, rhs)
+        return CudaBooleanBlock(out[:, 0], I)
+
+    def _scalar_compare(self, op, lhs, scalar) -> CudaBooleanBlock:
+        """`scalar` is one clear integer for every input, or one per input"""
+        from . import radix
+
+        kind, n, I = self._operands(lhs)
+        scalars = [scalar] * I if np.ndim(scalar) == 0 else list(scalar)
+        if len(scalars) != I:
+            raise ValueError(f"expected one scalar or {I}, got {len(scalars)}")
+        iconsts = radix.scalar_iconsts(scalars, n, kind.signed)
+        return CudaBooleanBlock(self._run(f"scalar_{op}", kind.signed, n, I, [lhs.blocks], iconsts)[:, 0], I)
+
+    def eq(self, lhs, rhs):
+        return self._compare("eq", lhs, rhs)
+
+    def ne(self, lhs, rhs):
+        return self._compare("ne", lhs, rhs)
+
+    def gt(self, lhs, rhs):
+        return self._compare("gt", lhs, rhs)
+
+    def ge(self, lhs, rhs):
+        return self._compare("ge", lhs, rhs)
+
+    def lt(self, lhs, rhs):
+        return self._compare("lt", lhs, rhs)
+
+    def le(self, lhs, rhs):
+        return self._compare("le", lhs, rhs)
+
+    def scalar_eq(self, lhs, scalar):
+        return self._scalar_compare("eq", lhs, scalar)
+
+    def scalar_ne(self, lhs, scalar):
+        return self._scalar_compare("ne", lhs, scalar)
+
+    def scalar_gt(self, lhs, scalar):
+        return self._scalar_compare("gt", lhs, scalar)
+
+    def scalar_ge(self, lhs, scalar):
+        return self._scalar_compare("ge", lhs, scalar)
+
+    def scalar_lt(self, lhs, scalar):
+        return self._scalar_compare("lt", lhs, scalar)
+
+    def scalar_le(self, lhs, scalar):
+        return self._scalar_compare("le", lhs, scalar)
+
+    def min(self, lhs, rhs):
+        kind, I, out = self._binary("min", lhs, rhs)
+        return self._radix(kind, out, I)
+
+    def max(self, lhs, rhs):
+        kind, I, out = self._binary("max", lhs, rhs)
+        return self._radix(kind, out, I)
+
+    def if_then_else(self, condition: CudaBooleanBlock, true_ct, false_ct):
+        """true_ct where the condition holds, else false_ct, per input"""
+        kind, n, I = self._operands(true_ct, false_ct)
+        if not isinstance(condition, CudaBooleanBlock) or condition.num_inputs != I \
+                or condition.blocks.shape[0] != I:
+            raise ValueError(f"the condition must be a CudaBooleanBlock of {I} input(s)")
+        out = self._run("if_then_else", False, n, I, [condition.blocks, true_ct.blocks, false_ct.blocks])
+        return self._radix(kind, out, I)
+
+    def add(self, lhs, rhs):
+        """lhs + rhs, wrapping mod 4^num_blocks"""
+        kind, I, out = self._binary("add", lhs, rhs)
+        return self._radix(kind, out, I)
+
+    def sub(self, lhs, rhs):
+        """lhs - rhs, wrapping mod 4^num_blocks"""
+        kind, I, out = self._binary("sub", lhs, rhs)
+        return self._radix(kind, out, I)
+
+    def neg(self, ct):
+        """-ct, wrapping mod 4^num_blocks"""
+        kind, n, I = self._operands(ct)
+        return self._radix(kind, self._run("neg", False, n, I, [ct.blocks]), I)
+
+    def _overflowing(self, op, lhs, rhs):
+        kind, n, I = self._operands(lhs, rhs)
+        if kind.signed:
+            raise ValueError(f"unsigned_{op} takes unsigned integers")
+        out = self._run(op, False, n, I, [lhs.blocks, rhs.blocks])
+        return self._radix(kind, out[:, :n], I), CudaBooleanBlock(out[:, n], I)
+
+    def unsigned_overflowing_add(self, lhs, rhs):
+        """(lhs + rhs wrapping, [lhs + rhs >= 4^num_blocks])"""
+        return self._overflowing("overflowing_add", lhs, rhs)
+
+    def unsigned_overflowing_sub(self, lhs, rhs):
+        """(lhs - rhs wrapping, [lhs < rhs])"""
+        return self._overflowing("overflowing_sub", lhs, rhs)
+
+    def bitand(self, lhs, rhs):
+        kind, I, out = self._binary("bitand", lhs, rhs)
+        return self._radix(kind, out, I)
+
+    def bitor(self, lhs, rhs):
+        kind, I, out = self._binary("bitor", lhs, rhs)
+        return self._radix(kind, out, I)
+
+    def bitxor(self, lhs, rhs):
+        kind, I, out = self._binary("bitxor", lhs, rhs)
+        return self._radix(kind, out, I)
+
+    def bitnot(self, ct):
+        kind, n, I = self._operands(ct)
+        return self._radix(kind, self._run("bitnot", False, n, I, [ct.blocks]), I)
+
+    def transfer(self, from_amount, to_amount, amount):
+        """erc7984's `transfer_whitepaper` on unsigned balances, in one
+        circuit: sent = amount if from_amount >= amount else 0; returns
+        (from_amount - sent, to_amount + sent)."""
+        kind, n, I = self._operands(from_amount, to_amount, amount)
+        if kind.signed:
+            raise ValueError("transfer takes unsigned integers")
+        out = self._run("transfer", False, n, I, [from_amount.blocks, to_amount.blocks, amount.blocks])
+        return self._radix(kind, out[:, :n], I), self._radix(kind, out[:, n:], I)

@@ -1,0 +1,122 @@
+#!/usr/bin/env python
+"""Cost of the radix-integer operations on one GPU (CUDA events, L2 flushed
+before every timed step, after one warm-up call), FheUint64 (32 blocks of
+2_2), classic PARAM_MESSAGE_2_CARRY_2 and multi-bit
+PARAM_GPU_MULTI_BIT_GROUP_4_MESSAGE_2_CARRY_2:
+
+  * latency of one input: eq, gt, signed lt, add, sub, min, if_then_else and
+    transfer (CudaRadixServerKey methods);
+  * throughput at 256 inputs (one call, bit-sliced): gt, add and transfer, in
+    operations/s and PBS/s;
+  * every call's PBS count and PBS layers;
+  * plain KS + PBS (cuda_keyswitch_lwe_ciphertext_vector_64_64_async +
+    cuda_[multi_bit_]programmable_bootstrap_64_async) of a batch the size of
+    the call's widest layer, for scale.
+
+Every call runs with the key's work stream as the caller's stream.
+Synthetic (random) keys and ciphertexts: the kernels' work does not depend on
+their values.  Correctness is covered by tests/test_radix.py.  Prints one
+JSON line per measurement, then the card's name and power limit."""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--throughput-inputs", type=int, default=256)
+    ap.add_argument("--reps", type=int, default=3)
+    args = ap.parse_args()
+    import torch
+
+    from bench import gpu_identity
+    from bench_trivium import plain_ks_pbs
+    from tfhe_rs_b200 import bit_circuit as bc, gpu, integer, lib, radix as R, server_key
+
+    L = lib()
+    streams = gpu.CudaStreams.new_single_gpu(0)
+    st, sp, dev = streams.streams[0], streams.ptr(0), streams.device(0)
+    flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > the 50 MB L2
+    rng = np.random.default_rng(64)
+    k, N, n_blocks = 1, 2048, 32
+    W = k * N + 1
+
+    def timed(fn, reps):
+        """mean device ms of `reps` steps after one warm-up, on stream st"""
+        with torch.cuda.stream(st):
+            fn()
+            st.synchronize()
+            ms = 0.0
+            for _ in range(reps):
+                flush_buf.zero_()
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record(st)
+                fn()
+                b.record(st)
+                b.synchronize()
+                ms += a.elapsed_time(b)
+        return ms / reps
+
+    def rand_blocks(rows):
+        with torch.cuda.stream(st):
+            return torch.from_numpy(rng.integers(0, 1 << 63, (rows, W))).to(dev)
+
+    for name, n, g, pbs_base_log, ks_base_log, ks_level in (("classic P22", 918, 1, 23, 4, 4),
+                                                           ("multi-bit g=4", 920, 4, 22, 3, 5)):
+        num_ggsw = n if g == 1 else (n // g) << g
+        h_bsk = rng.integers(0, 1 << 64, size=num_ggsw * 4 * N, dtype=np.uint64)
+        h_ksk = rng.integers(0, 1 << 64, size=k * N * ks_level * (n + 1), dtype=np.uint64)
+        skey = server_key.upload_server_key(h_bsk, h_ksk, n=n, k=k, N=N, pbs_base_log=pbs_base_log, pbs_level=1,
+                                            ks_base_log=ks_base_log, ks_level=ks_level, grouping_factor=g,
+                                            centered_ms=g == 1, streams=streams)
+        rk = integer.CudaRadixServerKey(skey, None, k, N)
+
+        def operands(inputs, signed=False):
+            kind = integer.CudaSignedRadixCiphertext if signed else integer.CudaUnsignedRadixCiphertext
+            return kind(rand_blocks(n_blocks * inputs), inputs)
+
+        def calls(inputs, which):
+            a, b, c = operands(inputs), operands(inputs), operands(inputs)
+            sa, sb = operands(inputs, True), operands(inputs, True)
+            cond = integer.CudaBooleanBlock(rand_blocks(inputs), inputs)
+            table = {
+                "eq": (("eq", False), lambda: rk.eq(a, b)),
+                "gt": (("gt", False), lambda: rk.gt(a, b)),
+                "signed lt": (("lt", True), lambda: rk.lt(sa, sb)),
+                "add": (("add", False), lambda: rk.add(a, b)),
+                "sub": (("sub", False), lambda: rk.sub(a, b)),
+                "min": (("min", False), lambda: rk.min(a, b)),
+                "if_then_else": (("if_then_else", False), lambda: rk.if_then_else(cond, a, b)),
+                "transfer": (("transfer", False), lambda: rk.transfer(a, b, c)),
+            }
+            return [(w,) + table[w] for w in which]
+
+        for mode, inputs, which in (("latency", 1, ["eq", "gt", "signed lt", "add", "sub", "min", "if_then_else",
+                                                    "transfer"]),
+                                    ("throughput", args.throughput_inputs, ["gt", "add", "transfer"])):
+            for what, (op, signed), fn in calls(inputs, which):
+                circ = R.circuit(op, n_blocks, signed)
+                s = bc.schedule(circ, inputs)
+                assert rk.runner.chunk_size(circ, inputs) == inputs
+                t = timed(fn, args.reps)
+                widest = max(s.layer_outputs(i) for i in range(s.num_layers))
+                rec = {"what": f"{what} FheUint64, {name}", "mode": mode, "num_inputs": inputs, "ms": t,
+                       "ops_per_s": inputs / t * 1e3, "pbs": s.pbs_count(), "pbs_layers": s.num_layers,
+                       "pbs_per_s": s.pbs_count() / t * 1e3, "widest_layer": widest,
+                       "plain_ks_pbs_widest_layer_ms": plain_ks_pbs(
+                           L, torch, gpu, streams, sp, skey, rk, timed, args.reps, rng, n, k, N, g,
+                           pbs_base_log, ks_base_log, ks_level, widest)}
+                print(json.dumps(rec), flush=True)
+        rk.runner.close()
+    print(json.dumps({"gpu": gpu_identity(0), "torch_device": torch.cuda.get_device_name(0)}))
+
+
+if __name__ == "__main__":
+    main()
