@@ -118,6 +118,64 @@ SIGNATURES = {
 }
 
 
+# name -> (restype, argtypes); exactly the declarations of include/tfhe_b200_zk.h
+# (zk-cuda-backend's C ABI, pointers to its structs typed as void *)
+_sz = C.c_size_t
+ZK_SIGNATURES = {
+    "affine_to_projective_g1_wrapper": (None, [vp, vp]),
+    "affine_to_projective_g2_wrapper": (None, [vp, vp]),
+    "projective_to_affine_g1_wrapper": (None, [vp, vp]),
+    "projective_to_affine_g2_wrapper": (None, [vp, vp]),
+    "g1_point_at_infinity_wrapper": (None, [vp]),
+    "g2_point_at_infinity_wrapper": (None, [vp]),
+    "g1_projective_point_at_infinity_wrapper": (None, [vp]),
+    "g2_projective_point_at_infinity_wrapper": (None, [vp]),
+    "g1_is_infinity_wrapper": (C.c_bool, [vp]),
+    "g2_is_infinity_wrapper": (C.c_bool, [vp]),
+    "g1_msm_unmanaged_wrapper_async": (None, [vp, u32, vp, vp, vp, u32, vp]),
+    "g2_msm_unmanaged_wrapper_async": (None, [vp, u32, vp, vp, vp, u32, vp]),
+    "pippenger_scratch_size_g1_wrapper": (_sz, [u32, u32]),
+    "pippenger_scratch_size_g2_wrapper": (_sz, [u32, u32]),
+    "g1_msm_managed_wrapper": (None, [vp, u32, vp, vp, vp, u32, C.c_bool, C.POINTER(u64)]),
+    "g2_msm_managed_wrapper": (None, [vp, u32, vp, vp, vp, u32, C.c_bool, C.POINTER(u64)]),
+    "g1_from_montgomery_wrapper": (None, [vp, vp]),
+    "g2_from_montgomery_wrapper": (None, [vp, vp]),
+    "fp_to_montgomery_wrapper": (None, [vp, vp]),
+    "fp_from_montgomery_wrapper": (None, [vp, vp]),
+    "g1_projective_from_montgomery_normalized_wrapper": (None, [vp, vp]),
+    "g2_projective_from_montgomery_normalized_wrapper": (None, [vp, vp]),
+    "is_on_curve_g1_wrapper": (C.c_bool, [vp]),
+    "is_on_curve_g2_wrapper": (C.c_bool, [vp]),
+    "scalar_modulus_limbs_wrapper": (None, [vp]),
+    "b200_last_msm_config": (C.c_char_p, []),
+    "b200_last_msm_combine_us": (C.c_double, []),
+}
+# the reference's zk library, when oracle/build_ref_zk.sh has been run
+REF_ZK_LIB_PATH = os.path.join(os.path.dirname(_HERE), "oracle", "_ref", "libzk_cuda_backend_ref.so")
+
+
+def _type_zk(dll: C.CDLL, missing_ok) -> C.CDLL:
+    """Type the ZK_SIGNATURES entry points of `dll`; a name for which
+    missing_ok(name) holds may be absent, any other missing one raises."""
+    for name, (res, args) in ZK_SIGNATURES.items():
+        try:
+            fn = getattr(dll, name)
+        except AttributeError:
+            if not missing_ok(name):
+                raise
+            continue
+        fn.restype = res
+        fn.argtypes = args
+    return dll
+
+
+def load_zk(path: str = REF_ZK_LIB_PATH) -> C.CDLL:
+    """dlopen the reference's zk-cuda-backend library (A/B and parity) and type
+    every entry point of include/tfhe_b200_zk.h; this engine's b200_ additions
+    may be absent."""
+    return _type_zk(C.CDLL(path), lambda name: name.startswith(ADDITIONS))
+
+
 def build(verbose: bool = False) -> str:
     """Compile the library for sm_90a with nvcc (cross-compiles without a GPU)."""
     cmd = ["make", "-C", CSRC, "all"]
@@ -174,5 +232,7 @@ def lib() -> C.CDLL:
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                 "or `make -C tfhe-rs_b200/csrc`. There is no CPU fallback for the PBS path."
             )
-        _lib = load(LIB_PATH, strict=is_product())
+        # another library driven through B200_LIB_PATH (the reference's
+        # tfhe-cuda-backend) need not export the zk ABI
+        _lib = _type_zk(load(LIB_PATH, strict=is_product()), lambda name: not is_product())
     return _lib

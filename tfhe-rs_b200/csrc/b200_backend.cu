@@ -1,10 +1,13 @@
 // b200_backend.cu -- the single translation unit of
 // libtfhe_cuda_backend_b200.so: device helpers, per-device tables and the
 // extern "C" entry points declared in include/tfhe_b200.h (same names and
-// signatures as tfhe-rs' backends/tfhe-cuda-backend C ABI).
+// signatures as tfhe-rs' backends/tfhe-cuda-backend C ABI), and those of
+// include/tfhe_b200_zk.h (backends/zk-cuda-backend's C ABI).
 //
-// There is NO CPU fallback anywhere in this file: every entry point launches
-// sm_90a kernels or aborts.
+// There is NO CPU fallback anywhere in this file: every compute entry point
+// launches sm_90a kernels or aborts.  The zk ABI's point and field helpers
+// are host functions by definition (the reference's are too); its MSMs run on
+// the GPU apart from the final combination of window sums (DESIGN §8k).
 #include "../../include/tfhe_b200.h"
 
 #include <algorithm>
@@ -35,6 +38,10 @@
 #include "pbs128.cuh"
 #include "keyswitch128.cuh"
 #include "bit_circuit.cuh"
+#include "msm.cuh"
+#include <chrono>
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 namespace b200 {
 
@@ -1102,6 +1109,217 @@ static void launch_pbs128(cudaStream_t st, uint32_t gpu_index, u128 *lwe_out,
          base_log, l, num_samples, centered_ms, ws, stride);
   t_last_pbs_kernel = r.name;
   B200_CHECK(cudaFreeAsync(ws, st));
+}
+
+// ===========================================================================
+// BLS12-446 multi-scalar multiplication (msm.cuh)
+// ===========================================================================
+static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// window size, task and segment sizes, and the scratch layout of one MSM
+struct MsmPlan {
+  int c;
+  uint32_t W, B, nb, task, S, L, count, max_tasks, max_tasks_per_bucket;
+  int end_bit;
+  size_t sort_temp, scan_temp;
+  // byte offsets: keys/values in and out, bucket [start, end), tasks per
+  // bucket and their scan, task -> bucket, task partial sums, segment totals
+  // and running sums, window sums, CUB temporary storage; then the total
+  size_t keys_in, vals_in, keys_out, vals_out, bounds, ntasks, toff, task_bucket, partial, seg_total, seg_run,
+      win, temp, bytes;
+};
+
+// c minimises W (n + 3 B): the mixed additions of the accumulation plus the
+// two additions per bucket of the reduction (with the bucket's share of the
+// tree).  G2 caps c lower: its buckets are twice as large.
+template <class A> static MsmPlan msm_plan(uint32_t n) {
+  using F = MsmField<A>;
+  using X = zk::Xyzz<F>;
+  MsmPlan p{};
+  const int cmax = std::is_same<F, Fp>::value ? 16 : 14;
+  double best = 0;
+  for (int c = 4; c <= cmax; c++) {
+    const double cost = zk::num_windows(c) * ((double)n + 3.0 * (double)(1u << (c - 1)));
+    if (c == 4 || cost < best)
+      best = cost, p.c = c;
+  }
+  p.W = (uint32_t)zk::num_windows(p.c);
+  p.B = 1u << (p.c - 1);
+  p.nb = p.W * p.B;
+  p.task = 8;
+  p.S = std::min<uint32_t>(p.B, MSM_MAX_SEGMENTS);
+  p.L = p.B / p.S;
+  B200_PANIC_IF_FALSE((uint64_t)n * p.W < (1ull << 31), "MSM error: n = %u is too large", n);
+  p.count = n * p.W;
+  p.max_tasks = p.count / p.task + std::min(p.nb, p.count) + 1;
+  p.max_tasks_per_bucket = (n + p.task - 1) / p.task;
+  p.end_bit = 32 - __builtin_clz(p.nb);
+  B200_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, p.sort_temp, (uint32_t *)nullptr, (uint32_t *)nullptr,
+                                             (uint32_t *)nullptr, (uint32_t *)nullptr, (int)p.count, 0,
+                                             p.end_bit));
+  B200_CHECK(cub::DeviceScan::ExclusiveSum(nullptr, p.scan_temp, (uint32_t *)nullptr, (uint32_t *)nullptr,
+                                           (int)(p.nb + 1)));
+  size_t at = 0;
+  auto take = [&at](size_t bytes) {
+    const size_t off = at;
+    at += align256(bytes);
+    return off;
+  };
+  p.keys_in = take(p.count * 4ull);
+  p.vals_in = take(p.count * 4ull);
+  p.keys_out = take(p.count * 4ull);
+  p.vals_out = take(p.count * 4ull);
+  p.bounds = take(2ull * p.nb * 4);
+  p.ntasks = take((p.nb + 1ull) * 4);
+  p.toff = take((p.nb + 1ull) * 4);
+  p.task_bucket = take(p.max_tasks * 4ull);
+  p.partial = take(p.max_tasks * sizeof(X));
+  p.seg_total = take((size_t)p.W * p.S * sizeof(X));
+  p.seg_run = take((size_t)p.W * p.S * sizeof(X));
+  p.win = take((size_t)p.W * sizeof(X));
+  p.temp = take(std::max(p.sort_temp, p.scan_temp));
+  p.bytes = at;
+  return p;
+}
+
+static thread_local char t_last_msm_config[256] = "";
+static thread_local double t_last_msm_combine_us = 0;
+
+// sum k_i P_i of n device points (Montgomery form) and scalars into
+// *h_result (host); scratch holds msm_plan<A>(n).bytes.  Synchronizes `st`.
+template <class A, class Proj>
+static void msm_run(cudaStream_t st, uint32_t gpu, Proj *h_result, const A *d_points, const Scalar *d_scalars,
+                    uint32_t n, void *scratch) {
+  using F = MsmField<A>;
+  using X = zk::Xyzz<F>;
+  const MsmPlan p = msm_plan<A>(n);
+  unsigned char *base = static_cast<unsigned char *>(scratch);
+  uint32_t *keys_in = (uint32_t *)(base + p.keys_in), *vals_in = (uint32_t *)(base + p.vals_in);
+  uint32_t *keys_out = (uint32_t *)(base + p.keys_out), *vals_out = (uint32_t *)(base + p.vals_out);
+  uint32_t *start = (uint32_t *)(base + p.bounds), *end = start + p.nb;
+  uint32_t *ntasks = (uint32_t *)(base + p.ntasks), *toff = (uint32_t *)(base + p.toff);
+  uint32_t *task_bucket = (uint32_t *)(base + p.task_bucket);
+  X *partial = (X *)(base + p.partial), *seg_total = (X *)(base + p.seg_total);
+  X *seg_run = (X *)(base + p.seg_run), *win = (X *)(base + p.win);
+  void *temp = base + p.temp;
+  constexpr uint32_t T = 128;
+  auto blocks = [](uint64_t threads) { return (uint32_t)((threads + T - 1) / T); };
+
+  launch(msm_digits_kernel, {blocks(n), T, 0, st, gpu}, d_scalars, n, p.c, keys_in, vals_in);
+  size_t temp_bytes = p.sort_temp;
+  B200_CHECK(cub::DeviceRadixSort::SortPairs(temp, temp_bytes, keys_in, keys_out, vals_in, vals_out, (int)p.count,
+                                             0, p.end_bit, st));
+  B200_CHECK(cudaMemsetAsync(start, 0, 2ull * p.nb * sizeof(uint32_t), st));
+  launch(msm_bucket_bounds_kernel, {blocks(p.count), T, 0, st, gpu}, keys_out, p.count, p.nb, start, end);
+  launch(msm_task_count_kernel, {blocks(p.nb + 1ull), T, 0, st, gpu}, start, end, p.nb, p.task, ntasks);
+  temp_bytes = p.scan_temp;
+  B200_CHECK(cub::DeviceScan::ExclusiveSum(temp, temp_bytes, ntasks, toff, (int)(p.nb + 1), st));
+  launch(msm_accumulate_kernel<A>, {blocks(p.max_tasks), T, 0, st, gpu}, d_points, vals_out, start, end, toff,
+         p.nb, p.task, p.max_tasks, partial, task_bucket);
+  for (uint32_t step = 1; step < p.max_tasks_per_bucket; step *= 2)
+    launch(msm_bucket_tree_kernel<F>, {blocks(p.max_tasks), T, 0, st, gpu}, partial, task_bucket, toff, p.nb,
+           p.max_tasks, step);
+  launch(msm_bucket_reduce_kernel<F>, {blocks((uint64_t)p.W * p.S), T, 0, st, gpu}, partial, toff, p.W, p.B, p.L,
+         seg_total, seg_run);
+  launch(msm_window_sum_kernel<F>, {p.W, p.S, 0, st, gpu}, seg_total, seg_run, p.S, p.L, win);
+  X h_win[zk::SCALAR_BITS / 4 + 1];
+  B200_CHECK(cudaMemcpyAsync(h_win, win, p.W * sizeof(X), cudaMemcpyDeviceToHost, st));
+  B200_CHECK(cudaStreamSynchronize(st));
+
+  // 5b. Horner over the windows on the host: sum_w 2^(c w) S_w
+  const auto t0 = std::chrono::steady_clock::now();
+  X acc;
+  zk::xyzz_set_identity(acc);
+  for (int w = (int)p.W - 1; w >= 0; w--) {
+    if (!zk::xyzz_is_identity(acc))
+      for (int i = 0; i < p.c; i++)
+        zk::xyzz_dbl(acc, acc);
+    zk::xyzz_add(acc, h_win[w]);
+  }
+  zk::xyzz_to_projective(*h_result, acc);
+  t_last_msm_combine_us =
+      std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
+  std::snprintf(t_last_msm_config, sizeof(t_last_msm_config),
+                "c=%d windows=%u task=%u segments=%u kernels=msm_digits_kernel,cub::DeviceRadixSort,"
+                "msm_bucket_bounds_kernel,msm_task_count_kernel,cub::DeviceScan,msm_accumulate_kernel,"
+                "msm_bucket_tree_kernel,msm_bucket_reduce_kernel,msm_window_sum_kernel",
+                p.c, p.W, p.task, p.S);
+}
+
+static void msm_check_gpu(uint32_t gpu_index) {
+  int count = 0;
+  B200_CHECK(cudaGetDeviceCount(&count));
+  B200_PANIC_IF_FALSE(gpu_index < (uint32_t)count, "MSM error: invalid gpu_index=%u (gpu_count=%d)", gpu_index,
+                      count);
+  set_device(gpu_index);
+}
+
+template <class A, class Proj>
+static void msm_unmanaged(cudaStream_t stream, uint32_t gpu_index, Proj *h_result, const A *d_points,
+                          const Scalar *d_scalars, uint32_t n, void *d_scratch) {
+  B200_PANIC_IF_FALSE(n > 0, "MSM error: n must be positive, got %u", n);
+  B200_PANIC_IF_FALSE(stream && h_result && d_points && d_scalars && d_scratch, "MSM error: null argument");
+  msm_check_gpu(gpu_index);
+  msm_run(stream, gpu_index, h_result, d_points, d_scalars, n, d_scratch);
+}
+
+// host arrays: points, scalars and scratch from the stream-ordered pool
+template <class A, class Proj>
+static void msm_managed(cudaStream_t stream, uint32_t gpu_index, Proj *result, const A *points,
+                        const Scalar *scalars, uint32_t n, bool points_in_montgomery, uint64_t *size_tracker) {
+  B200_PANIC_IF_FALSE(n > 0, "MSM error: n must be positive, got %u", n);
+  B200_PANIC_IF_FALSE(stream && result && points && scalars && size_tracker, "MSM error: null argument");
+  msm_check_gpu(gpu_index);
+  const size_t pb = (size_t)n * sizeof(A), sb = (size_t)n * sizeof(Scalar);
+  const size_t scratch_bytes = msm_plan<A>(n).bytes;
+  unsigned char *ws = nullptr;
+  const size_t bytes = align256(pb) + align256(sb) + scratch_bytes;
+  B200_CHECK(cudaMallocFromPoolAsync(&ws, bytes, workspace_pool(gpu_index), stream));
+  *size_tracker += bytes;
+  A *d_points = (A *)ws;
+  Scalar *d_scalars = (Scalar *)(ws + align256(pb));
+  B200_CHECK(cudaMemcpyAsync(d_points, points, pb, cudaMemcpyHostToDevice, stream));
+  B200_CHECK(cudaMemcpyAsync(d_scalars, scalars, sb, cudaMemcpyHostToDevice, stream));
+  if (!points_in_montgomery)
+    launch(msm_to_montgomery_kernel<A>, {(n + 127) / 128, 128, 0, stream, gpu_index}, d_points, n);
+  msm_run(stream, gpu_index, result, d_points, d_scalars, n, ws + align256(pb) + align256(sb));
+  B200_CHECK(cudaFreeAsync(ws, stream));
+  B200_CHECK(cudaStreamSynchronize(stream));
+}
+
+// (X / Z, Y / Z, 1) in normal form; with Z = 0, X and Y leave Montgomery form
+// and Z stays 0
+template <class Proj> static void projective_normalized(Proj *result, const Proj *point) {
+  B200_PANIC_IF_FALSE(result && point && result != point, "projective_from_montgomery: bad pointers");
+  *result = *point;
+  if (zk::fp_is_zero(point->Z)) {
+    zk::fp_from_montgomery(result->X, point->X);
+    zk::fp_from_montgomery(result->Y, point->Y);
+    return;
+  }
+  decltype(point->Z) zi;
+  zk::fp_inv(zi, point->Z);
+  zk::fp_mul(result->X, point->X, zi);
+  zk::fp_mul(result->Y, point->Y, zi);
+  zk::fp_from_montgomery(result->X, result->X);
+  zk::fp_from_montgomery(result->Y, result->Y);
+  zk::fp_zero(result->Z);
+  reinterpret_cast<Fp *>(&result->Z)->limb[0] = 1;  // 1, or 1 + 0 u
+}
+
+template <class A> static bool on_curve_normal(const A *point) {
+  B200_PANIC_IF_FALSE(point != nullptr, "is_on_curve: point is null");
+  if (point->infinity)
+    return true;
+  decltype(point->x) x, y;
+  zk::fp_to_montgomery(x, point->x);
+  zk::fp_to_montgomery(y, point->y);
+  return zk::on_curve_mont(x, y);
+}
+
+template <class A> static size_t msm_scratch_size(uint32_t n, uint32_t gpu_index) {
+  msm_check_gpu(gpu_index);
+  return msm_plan<A>(std::max<uint32_t>(n, 1)).bytes;
 }
 
 } // namespace b200
@@ -2545,6 +2763,155 @@ int b200_pbs_uses_fast_path(uint32_t lwe_dimension, uint32_t glwe_dimension,
 }
 
 const char *b200_version(void) { return "tfhe-rs_b200 0.1 (sm_90a)"; }
+
+// ===========================================================================
+// zk-cuda-backend C ABI (include/tfhe_b200_zk.h)
+// ===========================================================================
+void affine_to_projective_g1_wrapper(G1ProjectivePoint *proj, const G1Point *affine) {
+  if (affine->infinity) {
+    g1_projective_point_at_infinity_wrapper(proj);
+    return;
+  }
+  proj->X = affine->x, proj->Y = affine->y;
+  zk::fp_one(proj->Z);
+}
+
+void affine_to_projective_g2_wrapper(G2ProjectivePoint *proj, const G2Point *affine) {
+  if (affine->infinity) {
+    g2_projective_point_at_infinity_wrapper(proj);
+    return;
+  }
+  proj->X = affine->x, proj->Y = affine->y;
+  zk::fp_one(proj->Z);
+}
+
+void projective_to_affine_g1_wrapper(G1Point *affine, const G1ProjectivePoint *proj) {
+  if (zk::fp_is_zero(proj->Z)) {
+    g1_point_at_infinity_wrapper(affine);
+    return;
+  }
+  Fp zi;
+  zk::fp_inv(zi, proj->Z);
+  zk::fp_mul(affine->x, proj->X, zi);
+  zk::fp_mul(affine->y, proj->Y, zi);
+  affine->infinity = false;
+}
+
+void projective_to_affine_g2_wrapper(G2Point *affine, const G2ProjectivePoint *proj) {
+  if (zk::fp_is_zero(proj->Z)) {
+    g2_point_at_infinity_wrapper(affine);
+    return;
+  }
+  Fp2 zi;
+  zk::fp_inv(zi, proj->Z);
+  zk::fp_mul(affine->x, proj->X, zi);
+  zk::fp_mul(affine->y, proj->Y, zi);
+  affine->infinity = false;
+}
+
+void g1_point_at_infinity_wrapper(G1Point *point) {
+  std::memset(point, 0, sizeof(*point));
+  point->infinity = true;
+}
+
+void g2_point_at_infinity_wrapper(G2Point *point) {
+  std::memset(point, 0, sizeof(*point));
+  point->infinity = true;
+}
+
+void g1_projective_point_at_infinity_wrapper(G1ProjectivePoint *point) { std::memset(point, 0, sizeof(*point)); }
+
+void g2_projective_point_at_infinity_wrapper(G2ProjectivePoint *point) { std::memset(point, 0, sizeof(*point)); }
+
+bool g1_is_infinity_wrapper(const G1Point *point) { return point->infinity; }
+
+bool g2_is_infinity_wrapper(const G2Point *point) { return point->infinity; }
+
+void g1_msm_unmanaged_wrapper_async(cudaStream_t stream, uint32_t gpu_index, G1ProjectivePoint *h_result,
+                                    const G1Point *d_points, const Scalar *d_scalars, uint32_t n,
+                                    G1ProjectivePoint *d_scratch) {
+  msm_unmanaged(stream, gpu_index, h_result, d_points, d_scalars, n, d_scratch);
+}
+
+void g2_msm_unmanaged_wrapper_async(cudaStream_t stream, uint32_t gpu_index, G2ProjectivePoint *h_result,
+                                    const G2Point *d_points, const Scalar *d_scalars, uint32_t n,
+                                    G2ProjectivePoint *d_scratch) {
+  msm_unmanaged(stream, gpu_index, h_result, d_points, d_scalars, n, d_scratch);
+}
+
+size_t pippenger_scratch_size_g1_wrapper(uint32_t n, uint32_t gpu_index) {
+  return msm_scratch_size<G1Point>(n, gpu_index);
+}
+
+size_t pippenger_scratch_size_g2_wrapper(uint32_t n, uint32_t gpu_index) {
+  return msm_scratch_size<G2Point>(n, gpu_index);
+}
+
+void g1_msm_managed_wrapper(cudaStream_t stream, uint32_t gpu_index, G1ProjectivePoint *result,
+                            const G1Point *points, const Scalar *scalars, uint32_t n, bool points_in_montgomery,
+                            uint64_t *size_tracker) {
+  msm_managed(stream, gpu_index, result, points, scalars, n, points_in_montgomery, size_tracker);
+}
+
+void g2_msm_managed_wrapper(cudaStream_t stream, uint32_t gpu_index, G2ProjectivePoint *result,
+                            const G2Point *points, const Scalar *scalars, uint32_t n, bool points_in_montgomery,
+                            uint64_t *size_tracker) {
+  msm_managed(stream, gpu_index, result, points, scalars, n, points_in_montgomery, size_tracker);
+}
+
+void g1_from_montgomery_wrapper(G1Point *result, const G1Point *point) {
+  B200_PANIC_IF_FALSE(result && point && result != point, "g1_from_montgomery: bad pointers");
+  if (point->infinity) {
+    g1_point_at_infinity_wrapper(result);
+    return;
+  }
+  zk::fp_from_montgomery(result->x, point->x);
+  zk::fp_from_montgomery(result->y, point->y);
+  result->infinity = false;
+}
+
+void g2_from_montgomery_wrapper(G2Point *result, const G2Point *point) {
+  B200_PANIC_IF_FALSE(result && point && result != point, "g2_from_montgomery: bad pointers");
+  if (point->infinity) {
+    g2_point_at_infinity_wrapper(result);
+    return;
+  }
+  zk::fp_from_montgomery(result->x, point->x);
+  zk::fp_from_montgomery(result->y, point->y);
+  result->infinity = false;
+}
+
+void fp_to_montgomery_wrapper(Fp *result, const Fp *value) {
+  B200_PANIC_IF_FALSE(result && value && result != value, "fp_to_montgomery: bad pointers");
+  zk::fp_to_montgomery(*result, *value);
+}
+
+void fp_from_montgomery_wrapper(Fp *result, const Fp *value) {
+  B200_PANIC_IF_FALSE(result && value && result != value, "fp_from_montgomery: bad pointers");
+  zk::fp_from_montgomery(*result, *value);
+}
+
+void g1_projective_from_montgomery_normalized_wrapper(G1ProjectivePoint *result, const G1ProjectivePoint *point) {
+  projective_normalized(result, point);
+}
+
+void g2_projective_from_montgomery_normalized_wrapper(G2ProjectivePoint *result, const G2ProjectivePoint *point) {
+  projective_normalized(result, point);
+}
+
+bool is_on_curve_g1_wrapper(const G1Point *point) { return on_curve_normal(point); }
+
+bool is_on_curve_g2_wrapper(const G2Point *point) { return on_curve_normal(point); }
+
+void scalar_modulus_limbs_wrapper(uint64_t *limbs) {
+  B200_PANIC_IF_FALSE(limbs != nullptr, "scalar_modulus_limbs: limbs is null");
+  for (int i = 0; i < 5; i++)
+    limbs[i] = zk::r_limb(i);
+}
+
+const char *b200_last_msm_config(void) { return t_last_msm_config; }
+
+double b200_last_msm_combine_us(void) { return t_last_msm_combine_us; }
 
 } // extern "C"
 #pragma GCC visibility pop
