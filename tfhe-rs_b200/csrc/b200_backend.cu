@@ -186,32 +186,55 @@ static uint32_t ilog2_exact(uint32_t x) {
   return l;
 }
 
-// The same predicate picks the Fourier-BSK layout at key conversion and the
-// kernel at PBS time (cf. the reference's supports_specialized_2_2_params,
-// programmable_bootstrap_classic.cuh:198-212).
-static bool uses_fast_path(uint32_t n, uint32_t k, uint32_t N, uint32_t l) {
-  return N == 2048 && k == 1 && l == 1 && n <= 1024;
-}
+// The shape of a PBS: input LWE dimension n, GLWE dimension k, polynomial size
+// N, decomposition (base_log, l) and the multi-bit grouping factor, 1 for the
+// classic PBS.  Key conversion knows no base_log and leaves it 0.
+struct PbsParams {
+  uint32_t n, k, N, base_log, l, grouping;
+  PBS_TYPE type() const { return grouping > 1 ? MULTI_BIT : CLASSICAL; }
+  // GGSWs of the key: one per input coefficient, or 2^g per group of g
+  uint32_t num_ggsw() const { return grouping > 1 ? (n / grouping) << grouping : n; }
+};
 
-// (N = 512, l = 1, k <= 4, n <= 1024): register kernel of pbs_n512.cuh, e.g.
-// PARAM_MESSAGE_1_CARRY_1_KS_PBS.  Same predicate at key conversion and at PBS
-// time; B200_N512_GENERIC=1 keeps these shapes on the generic kernel (A/B).
-// b200_set_register_kernels(mask) switches them at run time (bit 0: N = 512,
-// bit 1: N = 8192); a key must be converted and used under the same setting.
+// register-kernel routes switched at run time: bit 0 the N = 512 kernel, bit 1
+// the N = 8192 kernel (b200_set_register_kernels; B200_N512_GENERIC=1 /
+// B200_N8192_GENERIC=1 clear them, read once per process).  Bits 2 and 3 pick
+// debug instances of the N = 8192 kernel (B200_N8192_GEN1,
+// B200_N8192_RACECHECK).
 static std::atomic<int> &register_kernel_mask() {
   static std::atomic<int> v((std::getenv("B200_N512_GENERIC") ? 0 : 1) | (std::getenv("B200_N8192_GENERIC") ? 0 : 2) |
                             (std::getenv("B200_N8192_GEN1") ? 4 : 0) | (std::getenv("B200_N8192_RACECHECK") ? 8 : 0));
   return v;
 }
-static bool uses_n512_path(uint32_t n, uint32_t k, uint32_t N, uint32_t l) {
-  return (register_kernel_mask().load() & 1) && N == 512 && l == 1 && k >= 1 && k <= 4 && n <= 1024;
-}
 
-// (N = 8192, k = 1, l = 2, n <= 2048): register kernel of pbs_n8192.cuh
-// (PARAM_MESSAGE_3_CARRY_3_KS_PBS).  B200_N8192_GENERIC=1 keeps the shape on the
-// global-workspace kernel (A/B; read at library load: it selects the key layout).
-static bool uses_n8192_path(uint32_t n, uint32_t k, uint32_t N, uint32_t l) {
-  return (register_kernel_mask().load() & 2) && N == 8192 && k == 1 && l == 2 && n <= 2048;
+// The kernel family a 64-bit PBS shape runs on.  The route also fixes the
+// Fourier-BSK layout, so key conversion and the PBS both ask pbs_route: a key
+// converted under one answer and bootstrapped under another decrypts to
+// garbage.  A key must therefore be converted and used under the same
+// b200_set_register_kernels setting.
+enum class PbsRoute { N2048, N8192, N512, MultiBitN2048, Generic };
+
+static PbsRoute pbs_route(const PbsParams &p) {
+  if (p.grouping > 1) {
+    // N = 2048, k = 1, l <= 2: the kernels of pbs_multibit_n2048.cuh.
+    // B200_MULTIBIT_GENERIC keeps every multi-bit shape on the generic kernel.
+    static const bool generic_only = std::getenv("B200_MULTIBIT_GENERIC") != nullptr;
+    return !generic_only && p.N == 2048 && p.k == 1 && p.l >= 1 && p.l <= 2 && p.grouping <= 4
+               ? PbsRoute::MultiBitN2048
+               : PbsRoute::Generic;
+  }
+  // cf. the reference's supports_specialized_2_2_params
+  // (programmable_bootstrap_classic.cuh:198-212)
+  if (p.N == 2048 && p.k == 1 && p.l == 1 && p.n <= 1024)
+    return PbsRoute::N2048;
+  const int mask = register_kernel_mask().load();
+  // pbs_n8192.cuh, PARAM_MESSAGE_3_CARRY_3_KS_PBS
+  if ((mask & 2) && p.N == 8192 && p.k == 1 && p.l == 2 && p.n <= 2048)
+    return PbsRoute::N8192;
+  // pbs_n512.cuh, e.g. PARAM_MESSAGE_1_CARRY_1_KS_PBS
+  if ((mask & 1) && p.N == 512 && p.l == 1 && p.k >= 1 && p.k <= 4 && p.n <= 1024)
+    return PbsRoute::N512;
+  return PbsRoute::Generic;
 }
 
 // B200_PBS_VARIANT pins a kernel for A/B measurements: 1 first-generation
@@ -284,14 +307,6 @@ static std::atomic<int> &n512_mode_sel() {
   return v;
 }
 
-// multi-bit twin of uses_fast_path (layout + kernel predicate)
-static bool uses_multibit_fast_path(uint32_t k, uint32_t N, uint32_t l,
-                                    uint32_t grouping) {
-  static const bool disabled = std::getenv("B200_MULTIBIT_GENERIC") != nullptr;
-  return !disabled && N == 2048 && k == 1 && l >= 1 && l <= 2 &&
-         grouping >= 2 && grouping <= 4;
-}
-
 static void check_polynomial_size(uint32_t N) {
   B200_PANIC_IF_FALSE(
       N >= 256 && N <= 16384 && (N & (N - 1)) == 0,
@@ -336,17 +351,35 @@ struct PbsScratch : public pbs_buffer_base_abi {
   ~PbsScratch() override { magic = 0; }
 };
 
-// (k, N, l) a scratch object is made for
-struct PbsShape {
-  uint32_t glwe_dim, poly_size, level_count;
-};
+// a new scratch object of `type` for (k, N, l), handed back through `buffer`.
+// The persistent kernels keep every intermediate on chip or in per-call
+// stream-ordered pool allocations: it holds no device workspace, whatever the
+// batch size, and the size returned is 0.
+static uint64_t new_pbs_scratch(int8_t **buffer, PBS_TYPE type, uint32_t k,
+                                uint32_t N, uint32_t l, uint32_t max_samples,
+                                bool allocate_gpu_memory, int centered_ms,
+                                bool torus128 = false) {
+  PbsScratch *s = new PbsScratch;
+  s->magic = SCRATCH_MAGIC;
+  s->type = type;
+  s->glwe_dim = k;
+  s->poly_size = N;
+  s->level_count = l;
+  s->max_samples = max_samples;
+  s->centered_ms = centered_ms;
+  s->gpu_memory_allocated = allocate_gpu_memory;
+  s->torus128 = torus128;
+  *buffer = reinterpret_cast<int8_t *>(s);
+  return 0;
+}
 
 // the scratch object behind `buffer`, checked to be a live one of `type` and of
-// the 128-bit PBS exactly when `torus128`; made for `shape` when one is given,
-// and for at least `samples` samples.  `what` names the caller in the messages.
+// the 128-bit PBS exactly when `torus128`; made for the (k, N, l) of `shape`
+// when one is given, and for at least `samples` samples.  `what` names the
+// caller in the messages.
 static const PbsScratch &pbs_scratch(const int8_t *buffer, PBS_TYPE type,
                                      const char *what,
-                                     std::optional<PbsShape> shape = {},
+                                     std::optional<PbsParams> shape = {},
                                      uint64_t samples = 0,
                                      bool torus128 = false) {
   const PbsScratch *s = reinterpret_cast<const PbsScratch *>(buffer);
@@ -356,9 +389,8 @@ static const PbsScratch &pbs_scratch(const int8_t *buffer, PBS_TYPE type,
                       "Cuda error (%s): the scratch buffer was made for the "
                       "%s PBS", what, s->torus128 ? "128-bit" : "64-bit");
   B200_PANIC_IF_FALSE(
-      !shape || (s->glwe_dim == shape->glwe_dim &&
-                 s->poly_size == shape->poly_size &&
-                 s->level_count == shape->level_count),
+      !shape || (s->glwe_dim == shape->k && s->poly_size == shape->N &&
+                 s->level_count == shape->l),
       "Cuda error (%s): scratch buffer was created for other parameters", what);
   B200_PANIC_IF_FALSE(samples <= s->max_samples,
                       "Cuda error (%s): scratch buffer made for %u samples, "
@@ -428,9 +460,9 @@ static void launch_multibit_ll(cudaStream_t stream, uint32_t gpu_index,
                                const uint64_t *luts, const uint64_t *lut_idx,
                                const uint64_t *lwe_in, const uint64_t *in_idx,
                                const cplx *bsk, const DeviceTables &t,
-                               uint32_t n, uint32_t base_log, uint32_t l,
-                               uint32_t grouping, uint32_t num_samples,
+                               const PbsParams &p, uint32_t num_samples,
                                uint32_t num_many_lut, uint32_t lut_stride) {
+  const uint32_t n = p.n, l = p.l, grouping = p.grouping;
   const uint32_t steps = n / grouping;
   const size_t bytes =
       (size_t)num_samples * steps * l * 4 * P22_M * sizeof(cplx);
@@ -467,7 +499,7 @@ static void launch_multibit_ll(cudaStream_t stream, uint32_t gpu_index,
   const auto &seq = seq_kernels[l == 1 && use_tma ? 2 : l - 1];
   launch(seq.kernel, {num_samples, 128, seq.smem, stream, gpu_index}, lwe_out,
          out_idx, luts, lut_idx, lwe_in, in_idx, bundle, t.fft1024, n, steps,
-         base_log, num_many_lut, lut_stride, multibit_ties_even().load());
+         p.base_log, num_many_lut, lut_stride, multibit_ties_even().load());
   t_last_pbs_kernel = seq.names[grouping - 2];
   B200_CHECK(cudaFreeAsync(bundle, stream));
 }
@@ -478,11 +510,15 @@ static void launch_pbs_generic(cudaStream_t stream, uint32_t gpu_index,
                                Torus *lwe_out, const Torus *out_idx,
                                const Torus *luts, const Torus *lut_idx,
                                const Torus *lwe_in, const Torus *in_idx,
-                               const void *bsk, uint32_t n, uint32_t k,
-                               uint32_t N, uint32_t base_log, uint32_t l,
-                               uint32_t grouping, uint32_t num_samples,
-                               uint32_t num_many_lut, uint32_t lut_stride,
-                               int centered_ms) {
+                               const void *bsk, const PbsParams &p,
+                               uint32_t num_samples, uint32_t num_many_lut,
+                               uint32_t lut_stride, int centered_ms) {
+  const uint32_t n = p.n, k = p.k, N = p.N, l = p.l, grouping = p.grouping;
+  if (grouping > 1) {
+    B200_PANIC_IF_FALSE(grouping <= 4 && n % grouping == 0,
+                        "Cuda error (multi-bit PBS): grouping factor must be "
+                        "2, 3 or 4 and divide the lwe dimension");
+  }
   const uint32_t logM = ilog2_exact(N) - 1;
   const DeviceTables &t = device_tables(gpu_index, logM);
   const size_t smem = generic_smem_bytes(grouping > 1 ? 16 : n, k, N, l);
@@ -511,7 +547,7 @@ static void launch_pbs_generic(cudaStream_t stream, uint32_t gpu_index,
     launch(pbs_generic_kernel<256, true, Torus>,
            {grid, 256, 0, stream, gpu_index}, lwe_out, out_idx, luts, lut_idx,
            lwe_in, in_idx, static_cast<const cplx *>(bsk), t.gen_tw[logM],
-           t.gen_root[logM], n, k, N, logM, base_log, l, grouping,
+           t.gen_root[logM], n, k, N, logM, p.base_log, l, grouping,
            num_many_lut, lut_stride, centered_ms, multibit_ties_even().load(),
            num_samples, ws, stride);
     t_last_pbs_kernel = std::is_same<Torus, uint32_t>::value
@@ -524,205 +560,251 @@ static void launch_pbs_generic(cudaStream_t stream, uint32_t gpu_index,
          {num_samples, 256, smem, stream, gpu_index, (size_t)max_dyn[gpu_index]},
          lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
          static_cast<const cplx *>(bsk), t.gen_tw[logM], t.gen_root[logM], n,
-         k, N, logM, base_log, l, grouping, num_many_lut, lut_stride,
+         k, N, logM, p.base_log, l, grouping, num_many_lut, lut_stride,
          centered_ms, multibit_ties_even().load(), 0, nullptr,
          0); // no workspace
   t_last_pbs_kernel =
       std::is_same<Torus, uint32_t>::value ? "generic_smem_u32" : "generic_smem";
 }
 
+// PbsRoute::N2048: N = 2048, k = 1, l = 1 (pbs_n2048.cuh)
+static void launch_n2048(cudaStream_t stream, uint32_t gpu_index,
+                         uint64_t *lwe_out, const uint64_t *out_idx,
+                         const uint64_t *luts, const uint64_t *lut_idx,
+                         const uint64_t *lwe_in, const uint64_t *in_idx,
+                         const void *bsk, const PbsParams &p,
+                         uint32_t num_samples, uint32_t num_many_lut,
+                         uint32_t lut_stride, int centered_ms) {
+  B200_PANIC_IF_FALSE(p.base_log <= 31, "Cuda error (PBS): base_log > 31");
+  const DeviceTables &t = device_tables(gpu_index, 0);
+  int variant = fast_variant();
+  if (p.base_log > 30) {
+    variant = 1; // v1's 64-bit accumulator holds base_log = 31
+  } else if (variant == 0 && num_samples <= sm_count(gpu_index)) {
+    // shipped, at most one CTA per SM: v6 with the whole key block of a step
+    // through the one-slot TMA ring (no key value is ever waited for) and
+    // exchange 2 through warp shuffles
+    variant = 19; // n2048_v6<0,true,2>
+  } else if (variant == 0) {
+    // shipped, two CTAs per SM: v6 hybrid -- own key row prefetched into
+    // registers, other row (the one v3 waited a full L2 round trip for)
+    // through the ring; rotate + decompose with the sign as a predicate
+    // (CVT = 2); lane-pair layout: each warp holds the same 16 threads of
+    // both polynomials (lanes l and l ^ 16), exchange 2 through half-warp
+    // shuffles, the other polynomial's spectrum taken with one shuffle in
+    // the MAC (no spectrum store, no barrier between the polynomials).
+    // Bit-identical to variant 17, the same instance in the 64-thread
+    // group layout.
+    variant = 20; // n2048_v6<2,true,2,1>
+  }
+  const N2048Instance &r = *n2048_instance(variant);
+  launch(r.kernel, {num_samples, 128, r.smem, stream, gpu_index}, lwe_out,
+         out_idx, luts, lut_idx, lwe_in, in_idx,
+         static_cast<const cplx *>(bsk), t.fft1024, p.n, p.base_log,
+         num_many_lut, lut_stride, centered_ms);
+  t_last_pbs_kernel = r.name;
+}
+
+// PbsRoute::N8192: N = 8192, k = 1, l = 2 (pbs_n8192.cuh)
+static void launch_n8192(cudaStream_t stream, uint32_t gpu_index,
+                         uint64_t *lwe_out, const uint64_t *out_idx,
+                         const uint64_t *luts, const uint64_t *lut_idx,
+                         const uint64_t *lwe_in, const uint64_t *in_idx,
+                         const void *bsk, const PbsParams &p,
+                         uint32_t num_samples, uint32_t num_many_lut,
+                         uint32_t lut_stride, int centered_ms) {
+  B200_PANIC_IF_FALSE(p.base_log * p.l <= 30,
+                      "Cuda error (PBS): base_log * level_count > 30 is not "
+                      "supported for N = 8192");
+  const DeviceTables &t = device_tables(gpu_index, 0);
+  const uint32_t grid = std::min(num_samples, sm_count(gpu_index));
+  // per-thread park area of the four spectra of a step (pbs_n8192.cuh)
+  cplx *park = nullptr;
+  B200_CHECK(cudaMallocFromPoolAsync(&park, (size_t)grid * P8K_PARK_PER_CTA * sizeof(cplx),
+                                     workspace_pool(gpu_index), stream));
+  // mask bit 2: the first-generation kernel (per-thread key loads), for A/B
+  if (register_kernel_mask().load() & 4) {
+    launch(pbs_n8192_k1_l2_kernel,
+           {grid, 256, sizeof(N8192Smem), stream, gpu_index}, lwe_out,
+           out_idx, luts, lut_idx, lwe_in, in_idx,
+           static_cast<const cplx *>(bsk), t.fft4096, p.n, p.base_log,
+           num_samples, num_many_lut, lut_stride, centered_ms,
+           multibit_ties_even().load(), park);
+    t_last_pbs_kernel = "n8192_v1";
+  } else {
+    static const uint32_t stagger = [] {
+      const char *e = std::getenv("B200_N8192_STAGGER");
+      return e ? (uint32_t)std::atoi(e) : 0u;
+    }();
+    // mask bit 3: the racecheck instance (every thread arrives on the ring's
+    // `empty` barriers itself)
+    const bool racecheck = register_kernel_mask().load() & 8;
+    launch(racecheck ? pbs_n8192_k1_l2_v2_kernel<true>
+                     : pbs_n8192_k1_l2_v2_kernel<false>,
+           {grid, 256, sizeof(N8192SmemV2), stream, gpu_index}, lwe_out,
+           out_idx, luts, lut_idx, lwe_in, in_idx,
+           static_cast<const cplx *>(bsk), t.fft4096, p.n, p.base_log,
+           num_samples, num_many_lut, lut_stride, centered_ms,
+           multibit_ties_even().load(), stagger, park);
+    t_last_pbs_kernel = racecheck ? "n8192_v2<true>" : "n8192_v2<false>";
+  }
+  B200_CHECK(cudaFreeAsync(park, stream));
+}
+
+// PbsRoute::N512: N = 512, l = 1, k <= 4 (pbs_n512.cuh)
+static void launch_n512(cudaStream_t stream, uint32_t gpu_index,
+                        uint64_t *lwe_out, const uint64_t *out_idx,
+                        const uint64_t *luts, const uint64_t *lut_idx,
+                        const uint64_t *lwe_in, const uint64_t *in_idx,
+                        const void *bsk, const PbsParams &p,
+                        uint32_t num_samples, uint32_t num_many_lut,
+                        uint32_t lut_stride, int centered_ms) {
+  B200_PANIC_IF_FALSE(p.base_log <= 31, "Cuda error (PBS): base_log > 31");
+  const uint32_t k = p.k;
+  const DeviceTables &t = device_tables(gpu_index, 0);
+  // B200_N512_MODE: 0 (default) TMA key ring, one CTA per SM, 1 / 2 / 3 LWEs
+  // per CTA by launch size; 2 / 3: ring with two / one LWE per CTA; 4: ring with
+  // three; 1: register key ring, two LWEs per CTA, two CTAs per SM
+  const int mode512 = n512_mode_sel().load();
+  // automatic: the fewest LWEs per CTA that still covers the launch in one
+  // round of the persistent grid (latency), three per CTA beyond that
+  // (throughput)
+  const uint32_t sms = sm_count(gpu_index);
+  const int per_cta = mode512 == 3 ? 1 : mode512 == 2 ? 2 : mode512 == 0 && num_samples <= sms ? 1
+                      : mode512 == 0 && num_samples <= 2 * sms ? 2 : 3;
+  // [k - 1][0: register key ring, two LWEs per CTA, two CTAs per SM;
+  //         G = 1, 2, 3: TMA key ring, G LWEs per CTA, one CTA per SM]
+  static const struct {
+    decltype(&pbs_n512_kernel<1, 1, true>) kernel;
+    size_t smem;
+    const char *name;
+  } n512_instances[4][4] = {
+      {{pbs_n512_kernel<1, 2, false>, sizeof(N512Smem<1, 2, false>), "n512<1,2,false>"},
+       {pbs_n512_kernel<1, 1, true>, sizeof(N512Smem<1, 1, true>), "n512<1,1,true>"},
+       {pbs_n512_kernel<1, 2, true>, sizeof(N512Smem<1, 2, true>), "n512<1,2,true>"},
+       {pbs_n512_kernel<1, 3, true>, sizeof(N512Smem<1, 3, true>), "n512<1,3,true>"}},
+      {{pbs_n512_kernel<2, 2, false>, sizeof(N512Smem<2, 2, false>), "n512<2,2,false>"},
+       {pbs_n512_kernel<2, 1, true>, sizeof(N512Smem<2, 1, true>), "n512<2,1,true>"},
+       {pbs_n512_kernel<2, 2, true>, sizeof(N512Smem<2, 2, true>), "n512<2,2,true>"},
+       {pbs_n512_kernel<2, 3, true>, sizeof(N512Smem<2, 3, true>), "n512<2,3,true>"}},
+      {{pbs_n512_kernel<3, 2, false>, sizeof(N512Smem<3, 2, false>), "n512<3,2,false>"},
+       {pbs_n512_kernel<3, 1, true>, sizeof(N512Smem<3, 1, true>), "n512<3,1,true>"},
+       {pbs_n512_kernel<3, 2, true>, sizeof(N512Smem<3, 2, true>), "n512<3,2,true>"},
+       {pbs_n512_kernel<3, 3, true>, sizeof(N512Smem<3, 3, true>), "n512<3,3,true>"}},
+      {{pbs_n512_kernel<4, 2, false>, sizeof(N512Smem<4, 2, false>), "n512<4,2,false>"},
+       {pbs_n512_kernel<4, 1, true>, sizeof(N512Smem<4, 1, true>), "n512<4,1,true>"},
+       {pbs_n512_kernel<4, 2, true>, sizeof(N512Smem<4, 2, true>), "n512<4,2,true>"},
+       {pbs_n512_kernel<4, 3, true>, sizeof(N512Smem<4, 3, true>), "n512<4,3,true>"}}};
+  const int col = mode512 == 1 ? 0 : per_cta;
+  const auto &r = n512_instances[k - 1][col];
+  const uint32_t G = col ? col : 2, ctas_per_sm = col ? 1 : 2;
+  // persistent grid (see the kernel)
+  const uint32_t grid = std::min((num_samples + G - 1) / G, ctas_per_sm * sms);
+  launch(r.kernel, {grid, 16 * (k + 1) * G, r.smem, stream, gpu_index},
+         lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
+         static_cast<const cplx *>(bsk), t.fft256, p.n, p.base_log, num_samples,
+         num_many_lut, lut_stride, centered_ms);
+  t_last_pbs_kernel = r.name;
+}
+
+// PbsRoute::MultiBitN2048: N = 2048, k = 1, l <= 2, grouping 2 to 4
+// (pbs_multibit_n2048.cuh)
+static void launch_multibit_n2048(cudaStream_t stream, uint32_t gpu_index,
+                                  uint64_t *lwe_out, const uint64_t *out_idx,
+                                  const uint64_t *luts, const uint64_t *lut_idx,
+                                  const uint64_t *lwe_in, const uint64_t *in_idx,
+                                  const void *bsk, const PbsParams &p,
+                                  uint32_t num_samples, uint32_t num_many_lut,
+                                  uint32_t lut_stride) {
+  B200_PANIC_IF_FALSE(p.n % p.grouping == 0,
+                      "Cuda error (multi-bit PBS): grouping factor must "
+                      "divide the lwe dimension");
+  B200_PANIC_IF_FALSE(p.base_log * p.l <= 31,
+                      "Cuda error (multi-bit PBS): base_log * level_count "
+                      "> 31 is not supported for N = 2048, k = 1");
+  const DeviceTables &t = device_tables(gpu_index, 10);
+  // low-latency mode for launches that cannot fill the GPU with the fused
+  // kernel: bundle for all groups at once, then the sequential products
+  if (num_samples <= multibit_ll_max_samples(gpu_index)) {
+    launch_multibit_ll(stream, gpu_index, lwe_out, out_idx, luts, lut_idx,
+                       lwe_in, in_idx, static_cast<const cplx *>(bsk), t, p,
+                       num_samples, num_many_lut, lut_stride);
+    return;
+  }
+  // [grouping - 2][l - 1]
+  static const struct {
+    decltype(&pbs_multibit_n2048_k1_kernel<2, 1>) kernel;
+    const char *name;
+  } fused_instances[3][2] = {
+      {{pbs_multibit_n2048_k1_kernel<2, 1>, "multibit_fused<2,1>"},
+       {pbs_multibit_n2048_k1_kernel<2, 2>, "multibit_fused<2,2>"}},
+      {{pbs_multibit_n2048_k1_kernel<3, 1>, "multibit_fused<3,1>"},
+       {pbs_multibit_n2048_k1_kernel<3, 2>, "multibit_fused<3,2>"}},
+      {{pbs_multibit_n2048_k1_kernel<4, 1>, "multibit_fused<4,1>"},
+       {pbs_multibit_n2048_k1_kernel<4, 2>, "multibit_fused<4,2>"}}};
+  const auto &r = fused_instances[p.grouping - 2][p.l - 1];
+  launch(r.kernel, {num_samples, 128, sizeof(MbSmem), stream, gpu_index},
+         lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
+         static_cast<const cplx *>(bsk), t.fft1024, t.gen_root[10],
+         t.mono2048, p.n, p.base_log, num_many_lut, lut_stride,
+         multibit_ties_even().load());
+  t_last_pbs_kernel = r.name;
+}
+
+// the 64-bit PBS of every entry point: checks shared by every route, then the
+// route's own checks and launch
 static void launch_pbs(cudaStream_t stream, uint32_t gpu_index,
                        uint64_t *lwe_out, const uint64_t *out_idx,
                        const uint64_t *luts, const uint64_t *lut_idx,
                        const uint64_t *lwe_in, const uint64_t *in_idx,
-                       const void *bsk, uint32_t n, uint32_t k, uint32_t N,
-                       uint32_t base_log, uint32_t l, uint32_t grouping,
+                       const void *bsk, const PbsParams &p,
                        uint32_t num_samples, uint32_t num_many_lut,
                        uint32_t lut_stride, int centered_ms) {
   if (num_samples == 0)
     return;
-  check_polynomial_size(N);
-  B200_PANIC_IF_FALSE(base_log * l <= 63 && base_log >= 1 && l >= 1,
+  check_polynomial_size(p.N);
+  B200_PANIC_IF_FALSE(p.base_log * p.l <= 63 && p.base_log >= 1 && p.l >= 1,
                       "Cuda error (PBS): base_log * level_count must be < 64");
   if (num_many_lut == 0)
     num_many_lut = 1;
-  const uint32_t logM = ilog2_exact(N) - 1;
-  if (grouping <= 1 && uses_fast_path(n, k, N, l)) {
-    B200_PANIC_IF_FALSE(base_log <= 31, "Cuda error (PBS): base_log > 31");
-    const DeviceTables &t = device_tables(gpu_index, 0);
-    int variant = fast_variant();
-    if (base_log > 30) {
-      variant = 1; // v1's 64-bit accumulator holds base_log = 31
-    } else if (variant == 0 && num_samples <= sm_count(gpu_index)) {
-      // shipped, at most one CTA per SM: v6 with the whole key block of a step
-      // through the one-slot TMA ring (no key value is ever waited for) and
-      // exchange 2 through warp shuffles
-      variant = 19; // n2048_v6<0,true,2>
-    } else if (variant == 0) {
-      // shipped, two CTAs per SM: v6 hybrid -- own key row prefetched into
-      // registers, other row (the one v3 waited a full L2 round trip for)
-      // through the ring; rotate + decompose with the sign as a predicate
-      // (CVT = 2); lane-pair layout: each warp holds the same 16 threads of
-      // both polynomials (lanes l and l ^ 16), exchange 2 through half-warp
-      // shuffles, the other polynomial's spectrum taken with one shuffle in
-      // the MAC (no spectrum store, no barrier between the polynomials).
-      // Bit-identical to variant 17, the same instance in the 64-thread
-      // group layout.
-      variant = 20; // n2048_v6<2,true,2,1>
-    }
-    const N2048Instance &r = *n2048_instance(variant);
-    launch(r.kernel, {num_samples, 128, r.smem, stream, gpu_index}, lwe_out,
-           out_idx, luts, lut_idx, lwe_in, in_idx,
-           static_cast<const cplx *>(bsk), t.fft1024, n, base_log,
-           num_many_lut, lut_stride, centered_ms);
-    t_last_pbs_kernel = r.name;
-    return;
+  switch (pbs_route(p)) {
+  case PbsRoute::N2048:
+    return launch_n2048(stream, gpu_index, lwe_out, out_idx, luts, lut_idx,
+                        lwe_in, in_idx, bsk, p, num_samples, num_many_lut,
+                        lut_stride, centered_ms);
+  case PbsRoute::N8192:
+    return launch_n8192(stream, gpu_index, lwe_out, out_idx, luts, lut_idx,
+                        lwe_in, in_idx, bsk, p, num_samples, num_many_lut,
+                        lut_stride, centered_ms);
+  case PbsRoute::N512:
+    return launch_n512(stream, gpu_index, lwe_out, out_idx, luts, lut_idx,
+                       lwe_in, in_idx, bsk, p, num_samples, num_many_lut,
+                       lut_stride, centered_ms);
+  case PbsRoute::MultiBitN2048:
+    return launch_multibit_n2048(stream, gpu_index, lwe_out, out_idx, luts,
+                                 lut_idx, lwe_in, in_idx, bsk, p, num_samples,
+                                 num_many_lut, lut_stride);
+  case PbsRoute::Generic:
+    return launch_pbs_generic<uint64_t>(stream, gpu_index, lwe_out, out_idx,
+                                        luts, lut_idx, lwe_in, in_idx, bsk, p,
+                                        num_samples, num_many_lut, lut_stride,
+                                        centered_ms);
   }
-  if (grouping <= 1 && uses_n8192_path(n, k, N, l)) {
-    B200_PANIC_IF_FALSE(base_log * l <= 30,
-                        "Cuda error (PBS): base_log * level_count > 30 is not "
-                        "supported for N = 8192");
-    const DeviceTables &t = device_tables(gpu_index, 0);
-    const uint32_t grid = std::min(num_samples, sm_count(gpu_index));
-    // per-thread park area of the four spectra of a step (pbs_n8192.cuh)
-    cplx *park = nullptr;
-    B200_CHECK(cudaMallocFromPoolAsync(&park, (size_t)grid * P8K_PARK_PER_CTA * sizeof(cplx),
-                                       workspace_pool(gpu_index), stream));
-    // mask bit 2: the first-generation kernel (per-thread key loads), for A/B
-    if (register_kernel_mask().load() & 4) {
-      launch(pbs_n8192_k1_l2_kernel,
-             {grid, 256, sizeof(N8192Smem), stream, gpu_index}, lwe_out,
-             out_idx, luts, lut_idx, lwe_in, in_idx,
-             static_cast<const cplx *>(bsk), t.fft4096, n, base_log,
-             num_samples, num_many_lut, lut_stride, centered_ms,
-             multibit_ties_even().load(), park);
-      t_last_pbs_kernel = "n8192_v1";
-    } else {
-      static const uint32_t stagger = [] {
-        const char *e = std::getenv("B200_N8192_STAGGER");
-        return e ? (uint32_t)std::atoi(e) : 0u;
-      }();
-      // mask bit 3: the racecheck instance (every thread arrives on the ring's
-      // `empty` barriers itself)
-      const bool racecheck = register_kernel_mask().load() & 8;
-      launch(racecheck ? pbs_n8192_k1_l2_v2_kernel<true>
-                       : pbs_n8192_k1_l2_v2_kernel<false>,
-             {grid, 256, sizeof(N8192SmemV2), stream, gpu_index}, lwe_out,
-             out_idx, luts, lut_idx, lwe_in, in_idx,
-             static_cast<const cplx *>(bsk), t.fft4096, n, base_log,
-             num_samples, num_many_lut, lut_stride, centered_ms,
-             multibit_ties_even().load(), stagger, park);
-      t_last_pbs_kernel = racecheck ? "n8192_v2<true>" : "n8192_v2<false>";
-    }
-    B200_CHECK(cudaFreeAsync(park, stream));
-    return;
-  }
-  if (grouping <= 1 && uses_n512_path(n, k, N, l)) {
-    B200_PANIC_IF_FALSE(base_log <= 31, "Cuda error (PBS): base_log > 31");
-    const DeviceTables &t = device_tables(gpu_index, 0);
-    // B200_N512_MODE: 0 (default) TMA key ring, one CTA per SM, 1 / 2 / 3 LWEs
-    // per CTA by launch size; 2 / 3: ring with two / one LWE per CTA; 4: ring with
-    // three; 1: register key ring, two LWEs per CTA, two CTAs per SM
-    const int mode512 = n512_mode_sel().load();
-    // automatic: the fewest LWEs per CTA that still covers the launch in one
-    // round of the persistent grid (latency), three per CTA beyond that
-    // (throughput)
-    const uint32_t sms = sm_count(gpu_index);
-    const int per_cta = mode512 == 3 ? 1 : mode512 == 2 ? 2 : mode512 == 0 && num_samples <= sms ? 1
-                        : mode512 == 0 && num_samples <= 2 * sms ? 2 : 3;
-    // [k - 1][0: register key ring, two LWEs per CTA, two CTAs per SM;
-    //         G = 1, 2, 3: TMA key ring, G LWEs per CTA, one CTA per SM]
-    static const struct {
-      decltype(&pbs_n512_kernel<1, 1, true>) kernel;
-      size_t smem;
-      const char *name;
-    } n512_instances[4][4] = {
-        {{pbs_n512_kernel<1, 2, false>, sizeof(N512Smem<1, 2, false>), "n512<1,2,false>"},
-         {pbs_n512_kernel<1, 1, true>, sizeof(N512Smem<1, 1, true>), "n512<1,1,true>"},
-         {pbs_n512_kernel<1, 2, true>, sizeof(N512Smem<1, 2, true>), "n512<1,2,true>"},
-         {pbs_n512_kernel<1, 3, true>, sizeof(N512Smem<1, 3, true>), "n512<1,3,true>"}},
-        {{pbs_n512_kernel<2, 2, false>, sizeof(N512Smem<2, 2, false>), "n512<2,2,false>"},
-         {pbs_n512_kernel<2, 1, true>, sizeof(N512Smem<2, 1, true>), "n512<2,1,true>"},
-         {pbs_n512_kernel<2, 2, true>, sizeof(N512Smem<2, 2, true>), "n512<2,2,true>"},
-         {pbs_n512_kernel<2, 3, true>, sizeof(N512Smem<2, 3, true>), "n512<2,3,true>"}},
-        {{pbs_n512_kernel<3, 2, false>, sizeof(N512Smem<3, 2, false>), "n512<3,2,false>"},
-         {pbs_n512_kernel<3, 1, true>, sizeof(N512Smem<3, 1, true>), "n512<3,1,true>"},
-         {pbs_n512_kernel<3, 2, true>, sizeof(N512Smem<3, 2, true>), "n512<3,2,true>"},
-         {pbs_n512_kernel<3, 3, true>, sizeof(N512Smem<3, 3, true>), "n512<3,3,true>"}},
-        {{pbs_n512_kernel<4, 2, false>, sizeof(N512Smem<4, 2, false>), "n512<4,2,false>"},
-         {pbs_n512_kernel<4, 1, true>, sizeof(N512Smem<4, 1, true>), "n512<4,1,true>"},
-         {pbs_n512_kernel<4, 2, true>, sizeof(N512Smem<4, 2, true>), "n512<4,2,true>"},
-         {pbs_n512_kernel<4, 3, true>, sizeof(N512Smem<4, 3, true>), "n512<4,3,true>"}}};
-    const int col = mode512 == 1 ? 0 : per_cta;
-    const auto &r = n512_instances[k - 1][col];
-    const uint32_t G = col ? col : 2, ctas_per_sm = col ? 1 : 2;
-    // persistent grid (see the kernel)
-    const uint32_t grid = std::min((num_samples + G - 1) / G, ctas_per_sm * sms);
-    launch(r.kernel, {grid, 16 * (k + 1) * G, r.smem, stream, gpu_index},
-           lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
-           static_cast<const cplx *>(bsk), t.fft256, n, base_log, num_samples,
-           num_many_lut, lut_stride, centered_ms);
-    t_last_pbs_kernel = r.name;
-    return;
-  }
-  if (grouping > 1 && uses_multibit_fast_path(k, N, l, grouping)) {
-    B200_PANIC_IF_FALSE(n % grouping == 0,
-                        "Cuda error (multi-bit PBS): grouping factor must "
-                        "divide the lwe dimension");
-    B200_PANIC_IF_FALSE(base_log * l <= 31,
-                        "Cuda error (multi-bit PBS): base_log * level_count "
-                        "> 31 is not supported for N = 2048, k = 1");
-    const DeviceTables &t = device_tables(gpu_index, 10);
-    // low-latency mode for launches that cannot fill the GPU with the fused
-    // kernel: bundle for all groups at once, then the sequential products
-    if (num_samples <= multibit_ll_max_samples(gpu_index)) {
-      launch_multibit_ll(stream, gpu_index, lwe_out, out_idx, luts, lut_idx,
-                         lwe_in, in_idx, static_cast<const cplx *>(bsk), t, n,
-                         base_log, l, grouping, num_samples, num_many_lut,
-                         lut_stride);
-      return;
-    }
-    // [grouping - 2][l - 1]
-    static const struct {
-      decltype(&pbs_multibit_n2048_k1_kernel<2, 1>) kernel;
-      const char *name;
-    } fused_instances[3][2] = {
-        {{pbs_multibit_n2048_k1_kernel<2, 1>, "multibit_fused<2,1>"},
-         {pbs_multibit_n2048_k1_kernel<2, 2>, "multibit_fused<2,2>"}},
-        {{pbs_multibit_n2048_k1_kernel<3, 1>, "multibit_fused<3,1>"},
-         {pbs_multibit_n2048_k1_kernel<3, 2>, "multibit_fused<3,2>"}},
-        {{pbs_multibit_n2048_k1_kernel<4, 1>, "multibit_fused<4,1>"},
-         {pbs_multibit_n2048_k1_kernel<4, 2>, "multibit_fused<4,2>"}}};
-    const auto &r = fused_instances[grouping - 2][l - 1];
-    launch(r.kernel, {num_samples, 128, sizeof(MbSmem), stream, gpu_index},
-           lwe_out, out_idx, luts, lut_idx, lwe_in, in_idx,
-           static_cast<const cplx *>(bsk), t.fft1024, t.gen_root[10],
-           t.mono2048, n, base_log, num_many_lut, lut_stride,
-           multibit_ties_even().load());
-    t_last_pbs_kernel = r.name;
-    return;
-  }
-  if (grouping > 1) {
-    B200_PANIC_IF_FALSE(grouping <= 4 && n % grouping == 0,
-                        "Cuda error (multi-bit PBS): grouping factor must be "
-                        "2, 3 or 4 and divide the lwe dimension");
-  }
-  launch_pbs_generic<uint64_t>(stream, gpu_index, lwe_out, out_idx, luts,
-                               lut_idx, lwe_in, in_idx, bsk, n, k, N, base_log,
-                               l, grouping, num_samples, num_many_lut,
-                               lut_stride, centered_ms);
 }
 
-// standard-domain BSK (device staging buffer) -> Fourier BSK in the engine's
-// layout
+// standard-domain BSK (device staging buffer) -> Fourier BSK in the layout of
+// `route`, the route the key's PBS takes.  The 32-bit torus has the generic
+// layout only: its entry points pass PbsRoute::Generic.
 template <typename Torus>
 static void convert_bsk_staged(cudaStream_t stream, uint32_t gpu_index,
-                               void *dest, const Torus *staging, uint32_t k,
-                               uint32_t N, uint32_t l, uint32_t num_ggsw,
-                               bool fast_layout, uint32_t multibit_grouping) {
+                               void *dest, const Torus *staging,
+                               const PbsParams &p, PbsRoute route) {
+  const uint32_t k = p.k, N = p.N, l = p.l;
   const uint32_t logM = ilog2_exact(N) - 1;
-  const size_t polys = (size_t)num_ggsw * l * (k + 1) * (k + 1);
-  const DeviceTables &t = device_tables(gpu_index, fast_layout ? 0 : logM);
+  const size_t polys = (size_t)p.num_ggsw() * l * (k + 1) * (k + 1);
+  const bool register_fft =
+      route == PbsRoute::N2048 || route == PbsRoute::MultiBitN2048;
+  const DeviceTables &t = device_tables(gpu_index, register_fft ? 0 : logM);
   cplx *out = static_cast<cplx *>(dest);
   // limit: the shared memory of the largest N, 16384
   const auto generic = [&] {
@@ -731,47 +813,46 @@ static void convert_bsk_staged(cudaStream_t stream, uint32_t gpu_index,
             (16384 / 2) * sizeof(cplx)},
            out, staging, t.gen_tw[logM], N, logM);
   };
-  if constexpr (std::is_same<Torus, uint32_t>::value)
-    generic(); // the only layout of the 32-bit torus
-  else if (multibit_grouping > 1 && fast_layout)
-    launch(bsk_convert_multibit_n2048_kernel,
-           {(unsigned)polys, 64, 0, stream, gpu_index}, out, staging,
-           t.fft1024, l, multibit_grouping);
-  else if (multibit_grouping > 1)
-    // every other multi-bit shape runs on the generic kernel, whatever its
-    // GGSW count: the classic register layouts below must not take it
+  if constexpr (std::is_same<Torus, uint32_t>::value) {
     generic();
-  else if (fast_layout)
-    launch(bsk_convert_n2048_k1_l1_kernel,
-           {(unsigned)polys, 64, 0, stream, gpu_index}, out, staging,
-           t.fft1024);
-  else if (uses_n8192_path(num_ggsw, k, N, l))
-    launch(bsk_convert_n8192_kernel,
-           {(unsigned)polys, 256, P8K_M * sizeof(cplx), stream, gpu_index},
-           out, staging, t.fft4096);
-  else if (uses_n512_path(num_ggsw, k, N, l))
-    launch(bsk_convert_n512_kernel,
-           {(unsigned)((polys + 1) / 2), 32, 0, stream, gpu_index}, out,
-           staging, t.fft256, k + 1, (uint32_t)polys);
-  else
-    generic();
+  } else {
+    switch (route) {
+    case PbsRoute::N2048:
+      return launch(bsk_convert_n2048_k1_l1_kernel,
+                    {(unsigned)polys, 64, 0, stream, gpu_index}, out, staging,
+                    t.fft1024);
+    case PbsRoute::N8192:
+      return launch(bsk_convert_n8192_kernel,
+                    {(unsigned)polys, 256, P8K_M * sizeof(cplx), stream,
+                     gpu_index},
+                    out, staging, t.fft4096);
+    case PbsRoute::N512:
+      return launch(bsk_convert_n512_kernel,
+                    {(unsigned)((polys + 1) / 2), 32, 0, stream, gpu_index},
+                    out, staging, t.fft256, k + 1, (uint32_t)polys);
+    case PbsRoute::MultiBitN2048:
+      return launch(bsk_convert_multibit_n2048_kernel,
+                    {(unsigned)polys, 64, 0, stream, gpu_index}, out, staging,
+                    t.fft1024, l, p.grouping);
+    case PbsRoute::Generic:
+      return generic();
+    }
+  }
 }
 
-// host standard-domain BSK -> device Fourier BSK in the engine's layout
+// host standard-domain BSK -> device Fourier BSK in the layout of `route`
 template <typename Torus>
 static void convert_bsk(cudaStream_t stream, uint32_t gpu_index, void *dest,
-                        const void *src_host, uint32_t k, uint32_t N,
-                        uint32_t l, uint32_t num_ggsw, bool fast_layout,
-                        uint32_t multibit_grouping = 0) {
-  check_polynomial_size(N);
-  const size_t polys = (size_t)num_ggsw * l * (k + 1) * (k + 1);
-  const size_t bytes = polys * N * sizeof(Torus);
+                        const void *src_host, const PbsParams &p,
+                        PbsRoute route) {
+  check_polynomial_size(p.N);
+  const size_t polys = (size_t)p.num_ggsw() * p.l * (p.k + 1) * (p.k + 1);
+  const size_t bytes = polys * p.N * sizeof(Torus);
   Torus *staging = nullptr;
   B200_CHECK(cudaMallocAsync(&staging, bytes, stream));
   B200_CHECK(cudaMemcpyAsync(staging, src_host, bytes, cudaMemcpyHostToDevice,
                              stream));
-  convert_bsk_staged<Torus>(stream, gpu_index, dest, staging, k, N, l,
-                            num_ggsw, fast_layout, multibit_grouping);
+  convert_bsk_staged<Torus>(stream, gpu_index, dest, staging, p, route);
   B200_CHECK(cudaFreeAsync(staging, stream));
 }
 
@@ -828,9 +909,8 @@ static void convert_seeded_bsk(cudaStream_t stream, uint32_t gpu_index,
                                void *dest, const void *bodies_host,
                                const uint8_t aes_key[16], uint64_t ctr_lo,
                                uint64_t ctr_hi, uint32_t first_byte_index,
-                               uint32_t k, uint32_t N, uint32_t l,
-                               uint32_t num_ggsw, bool fast_layout,
-                               uint32_t multibit_grouping) {
+                               const PbsParams &p, PbsRoute route) {
+  const uint32_t k = p.k, N = p.N;
   check_polynomial_size(N);
   B200_PANIC_IF_FALSE(first_byte_index == 0 || first_byte_index == 8,
                       "Cuda error (seeded key): the mask stream must start on "
@@ -839,7 +919,7 @@ static void convert_seeded_bsk(cudaStream_t stream, uint32_t gpu_index,
   const AesTables *tables = aes_device_tables(gpu_index);
   AesCtrKey key;
   aes_expand_key(aes_key, aes_host_tables(), key);
-  const uint64_t rows = (uint64_t)num_ggsw * l * (k + 1);
+  const uint64_t rows = (uint64_t)p.num_ggsw() * p.l * (k + 1);
   const size_t std_bytes = rows * (k + 1) * N * sizeof(uint64_t);
   const size_t body_bytes = rows * N * sizeof(uint64_t);
   uint64_t *staging = nullptr, *bodies = nullptr;
@@ -850,8 +930,7 @@ static void convert_seeded_bsk(cudaStream_t stream, uint32_t gpu_index,
   launch(seeded_bsk_expand_kernel,
          {sm_count(gpu_index) * 8, 256, 0, stream, gpu_index}, staging, bodies,
          tables, key, ctr_lo, ctr_hi, first_byte_index / 8, rows, k, N);
-  convert_bsk_staged(stream, gpu_index, dest, staging, k, N, l, num_ggsw,
-                     fast_layout, multibit_grouping);
+  convert_bsk_staged(stream, gpu_index, dest, staging, p, route);
   B200_CHECK(cudaFreeAsync(bodies, stream));
   B200_CHECK(cudaFreeAsync(staging, stream));
 }
@@ -1499,10 +1578,9 @@ void cuda_convert_lwe_programmable_bootstrap_key_64_async(
     uint32_t input_lwe_dim, uint32_t glwe_dim, uint32_t level_count,
     uint32_t polynomial_size) {
   set_device(gpu_index);
+  const PbsParams p{input_lwe_dim, glwe_dim, polynomial_size, 0, level_count, 1};
   convert_bsk<uint64_t>(static_cast<cudaStream_t>(stream), gpu_index, dest, src,
-                        glwe_dim, polynomial_size, level_count, input_lwe_dim,
-                        uses_fast_path(input_lwe_dim, glwe_dim,
-                                       polynomial_size, level_count));
+                        p, pbs_route(p));
 }
 
 uint64_t scratch_cuda_programmable_bootstrap_64_async(
@@ -1513,26 +1591,18 @@ uint64_t scratch_cuda_programmable_bootstrap_64_async(
   (void)stream;
   set_device(gpu_index);
   check_polynomial_size(polynomial_size);
-  PbsScratch *s = new PbsScratch;
-  s->magic = SCRATCH_MAGIC;
-  s->type = CLASSICAL;
-  s->glwe_dim = glwe_dimension;
-  s->poly_size = polynomial_size;
-  s->level_count = level_count;
-  s->max_samples = input_lwe_ciphertext_count;
-  s->centered_ms = noise_reduction_type == CENTERED;
-  s->gpu_memory_allocated = allocate_gpu_memory;
   // per-device constant tables are built here (set-up call), so that the
-  // *_async bootstrap itself never runs a synchronous copy
-  device_tables(gpu_index,
-                uses_fast_path(lwe_dimension, glwe_dimension, polynomial_size,
-                               level_count)
-                    ? 0
-                    : ilog2_exact(polynomial_size) - 1);
-  *buffer = reinterpret_cast<int8_t *>(s);
-  // The persistent kernels keep every intermediate in shared memory /
-  // registers: no device workspace is needed, whatever the batch size.
-  return 0;
+  // *_async bootstrap itself never runs a synchronous copy: the register
+  // tables on the N = 2048 route, the generic ones for every other shape,
+  // whatever its route (the 32-bit PBS runs the generic kernel on this
+  // scratch object)
+  const PbsParams p{lwe_dimension, glwe_dimension, polynomial_size, 0, level_count, 1};
+  device_tables(gpu_index, pbs_route(p) == PbsRoute::N2048
+                               ? 0
+                               : ilog2_exact(polynomial_size) - 1);
+  return new_pbs_scratch(buffer, CLASSICAL, glwe_dimension, polynomial_size,
+                         level_count, input_lwe_ciphertext_count,
+                         allocate_gpu_memory, noise_reduction_type == CENTERED);
 }
 
 void cuda_programmable_bootstrap_64_async(
@@ -1544,9 +1614,8 @@ void cuda_programmable_bootstrap_64_async(
     uint32_t polynomial_size, uint32_t base_log, uint32_t level_count,
     uint32_t num_samples, uint32_t num_many_lut, uint32_t lut_stride) {
   set_device(gpu_index);
-  const PbsScratch &s =
-      pbs_scratch(buffer, CLASSICAL, "classical PBS",
-                  PbsShape{glwe_dimension, polynomial_size, level_count});
+  const PbsParams p{lwe_dimension, glwe_dimension, polynomial_size, base_log, level_count, 1};
+  const PbsScratch &s = pbs_scratch(buffer, CLASSICAL, "classical PBS", p);
   B200_PANIC_IF_FALSE(base_log <= 64,
                       "Cuda error (classical PBS): base log should be <= 64");
   launch_pbs(static_cast<cudaStream_t>(stream), gpu_index,
@@ -1556,8 +1625,7 @@ void cuda_programmable_bootstrap_64_async(
              static_cast<const uint64_t *>(lut_vector_indexes),
              static_cast<const uint64_t *>(lwe_array_in),
              static_cast<const uint64_t *>(lwe_input_indexes),
-             bootstrapping_key, lwe_dimension, glwe_dimension, polynomial_size,
-             base_log, level_count, 1, num_samples, num_many_lut, lut_stride,
+             bootstrapping_key, p, num_samples, num_many_lut, lut_stride,
              s.centered_ms);
 }
 
@@ -1581,15 +1649,18 @@ void cleanup_cuda_programmable_bootstrap_64(void *stream, uint32_t gpu_index,
 // The reference has no scratch function for the 32-bit PBS (its buffer type is
 // only reachable from C++): the `buffer` argument here is a scratch object of
 // scratch_cuda_programmable_bootstrap_64_async with the same (k, N, l).  Key,
-// ciphertexts, accumulators and the three index vectors are all u32.
+// ciphertexts, accumulators and the three index vectors are all u32.  The
+// 32-bit torus has one route whatever the shape: the generic key layout and
+// kernel.
 void cuda_convert_lwe_programmable_bootstrap_key_32_async(
     void *stream, uint32_t gpu_index, void *dest, void const *src,
     uint32_t input_lwe_dim, uint32_t glwe_dim, uint32_t level_count,
     uint32_t polynomial_size) {
   set_device(gpu_index);
   convert_bsk<uint32_t>(static_cast<cudaStream_t>(stream), gpu_index, dest, src,
-                        glwe_dim, polynomial_size, level_count, input_lwe_dim,
-                        false);
+                        PbsParams{input_lwe_dim, glwe_dim, polynomial_size, 0,
+                                  level_count, 1},
+                        PbsRoute::Generic);
 }
 
 void cuda_programmable_bootstrap_lwe_ciphertext_vector_32_async(
@@ -1615,7 +1686,8 @@ void cuda_programmable_bootstrap_lwe_ciphertext_vector_32_async(
       static_cast<const uint32_t *>(lut_vector_indexes),
       static_cast<const uint32_t *>(lwe_array_in),
       static_cast<const uint32_t *>(lwe_input_indexes), bootstrapping_key,
-      lwe_dimension, glwe_dimension, polynomial_size, base_log, level_count, 1,
+      PbsParams{lwe_dimension, glwe_dimension, polynomial_size, base_log,
+                level_count, 1},
       num_samples, num_many_lut ? num_many_lut : 1, lut_stride, s.centered_ms);
 }
 
@@ -1651,22 +1723,13 @@ uint64_t scratch_cuda_programmable_bootstrap_128_async(
   (void)lwe_dimension;
   set_device(gpu_index);
   pbs128_instance(glwe_dimension, polynomial_size, level_count, 1);
-  PbsScratch *s = new PbsScratch;
-  s->magic = SCRATCH_MAGIC;
-  s->type = CLASSICAL;
-  s->glwe_dim = glwe_dimension;
-  s->poly_size = polynomial_size;
-  s->level_count = level_count;
-  s->max_samples = input_lwe_ciphertext_count;
-  s->centered_ms = noise_reduction_type == CENTERED;
-  s->gpu_memory_allocated = allocate_gpu_memory;
-  s->torus128 = true;
   // the twiddle table is built here (set-up call), so that the bootstrap
   // itself never runs a synchronous copy
   dd_twiddles(gpu_index, ilog2_exact(polynomial_size) - 1);
-  *buffer = reinterpret_cast<int8_t *>(s);
-  // the per-call workspace is a stream-ordered pool allocation of the PBS
-  return 0;
+  return new_pbs_scratch(buffer, CLASSICAL, glwe_dimension, polynomial_size,
+                         level_count, input_lwe_ciphertext_count,
+                         allocate_gpu_memory, noise_reduction_type == CENTERED,
+                         true);
 }
 
 void cuda_programmable_bootstrap_128_async(
@@ -1678,7 +1741,8 @@ void cuda_programmable_bootstrap_128_async(
   set_device(gpu_index);
   const PbsScratch &s =
       pbs_scratch(buffer, CLASSICAL, "128-bit PBS",
-                  PbsShape{glwe_dimension, polynomial_size, level_count},
+                  PbsParams{lwe_dimension, glwe_dimension, polynomial_size,
+                            base_log, level_count, 1},
                   num_samples, true);
   launch_pbs128(static_cast<cudaStream_t>(stream), gpu_index,
                 static_cast<u128 *>(lwe_array_out),
@@ -1718,14 +1782,21 @@ void cuda_convert_lwe_multi_bit_programmable_bootstrap_key_64_async(
   B200_PANIC_IF_FALSE(grouping_factor >= 1 && grouping_factor <= 4 &&
                           input_lwe_dim % grouping_factor == 0,
                       "Cuda error (multi-bit PBS): unsupported grouping factor");
-  const uint32_t num_ggsw = (input_lwe_dim / grouping_factor)
-                            << grouping_factor;
-  const bool mb_fast = grouping_factor >= 2 &&
-                       uses_multibit_fast_path(glwe_dim, polynomial_size,
-                                               level_count, grouping_factor);
+  if (grouping_factor == 1) {
+    // No PBS reads such a key (the multi-bit PBS rejects grouping 1).  Its
+    // 2n GGSWs keep the layout of a classic key of 2n GGSWs, the N = 2048
+    // register layout excepted.
+    const PbsParams p{2 * input_lwe_dim, glwe_dim, polynomial_size, 0, level_count, 1};
+    const PbsRoute route = pbs_route(p);
+    convert_bsk<uint64_t>(static_cast<cudaStream_t>(stream), gpu_index, dest,
+                          src, p,
+                          route == PbsRoute::N2048 ? PbsRoute::Generic : route);
+    return;
+  }
+  const PbsParams p{input_lwe_dim, glwe_dim, polynomial_size, 0, level_count,
+                    grouping_factor};
   convert_bsk<uint64_t>(static_cast<cudaStream_t>(stream), gpu_index, dest, src,
-                        glwe_dim, polynomial_size, level_count, num_ggsw,
-                        mb_fast, grouping_factor);
+                        p, pbs_route(p));
 }
 
 void b200_convert_seeded_lwe_programmable_bootstrap_key_64_async(
@@ -1738,24 +1809,11 @@ void b200_convert_seeded_lwe_programmable_bootstrap_key_64_async(
                           (grouping_factor <= 1 ||
                            input_lwe_dim % grouping_factor == 0),
                       "Cuda error (seeded key): unsupported grouping factor");
-  if (grouping_factor <= 1) {
-    convert_seeded_bsk(static_cast<cudaStream_t>(stream), gpu_index, dest,
-                       seeded_bodies, aes_key, counter_lo, counter_hi,
-                       first_byte_index, glwe_dim, polynomial_size, level_count,
-                       input_lwe_dim,
-                       uses_fast_path(input_lwe_dim, glwe_dim, polynomial_size,
-                                      level_count),
-                       0);
-    return;
-  }
-  const uint32_t num_ggsw = (input_lwe_dim / grouping_factor)
-                            << grouping_factor;
-  const bool mb_fast = uses_multibit_fast_path(glwe_dim, polynomial_size,
-                                               level_count, grouping_factor);
+  const PbsParams p{input_lwe_dim, glwe_dim, polynomial_size, 0, level_count,
+                    std::max(grouping_factor, 1u)};
   convert_seeded_bsk(static_cast<cudaStream_t>(stream), gpu_index, dest,
                      seeded_bodies, aes_key, counter_lo, counter_hi,
-                     first_byte_index, glwe_dim, polynomial_size, level_count,
-                     num_ggsw, mb_fast, grouping_factor);
+                     first_byte_index, p, pbs_route(p));
 }
 
 uint64_t scratch_cuda_multi_bit_programmable_bootstrap_64_async(
@@ -1765,18 +1823,10 @@ uint64_t scratch_cuda_multi_bit_programmable_bootstrap_64_async(
   (void)stream;
   set_device(gpu_index);
   check_polynomial_size(polynomial_size);
-  PbsScratch *s = new PbsScratch;
-  s->magic = SCRATCH_MAGIC;
-  s->type = MULTI_BIT;
-  s->glwe_dim = glwe_dimension;
-  s->poly_size = polynomial_size;
-  s->level_count = level_count;
-  s->max_samples = input_lwe_ciphertext_count;
-  s->centered_ms = 0;
-  s->gpu_memory_allocated = allocate_gpu_memory;
   device_tables(gpu_index, ilog2_exact(polynomial_size) - 1);
-  *pbs_buffer = reinterpret_cast<int8_t *>(s);
-  return 0;
+  return new_pbs_scratch(pbs_buffer, MULTI_BIT, glwe_dimension,
+                         polynomial_size, level_count,
+                         input_lwe_ciphertext_count, allocate_gpu_memory, 0);
 }
 
 void cuda_multi_bit_programmable_bootstrap_64_async(
@@ -1801,9 +1851,10 @@ void cuda_multi_bit_programmable_bootstrap_64_async(
              static_cast<const uint64_t *>(lut_vector_indexes),
              static_cast<const uint64_t *>(lwe_array_in),
              static_cast<const uint64_t *>(lwe_input_indexes),
-             bootstrapping_key, lwe_dimension, glwe_dimension, polynomial_size,
-             base_log, level_count, grouping_factor, num_samples, num_many_lut,
-             lut_stride, 0);
+             bootstrapping_key,
+             PbsParams{lwe_dimension, glwe_dimension, polynomial_size, base_log,
+                       level_count, grouping_factor},
+             num_samples, num_many_lut, lut_stride, 0);
 }
 
 void cleanup_cuda_multi_bit_programmable_bootstrap_64(void *stream,
@@ -2110,9 +2161,9 @@ void b200_grouped_oprf_64_async(
     uint32_t level_count, uint32_t grouping_factor, uint32_t num_blocks) {
   set_device(gpu_index);
   check_polynomial_size(polynomial_size);
-  const bool multi_bit = grouping_factor > 1;
-  pbs_scratch(buffer, multi_bit ? MULTI_BIT : CLASSICAL, "OPRF",
-              PbsShape{glwe_dimension, polynomial_size, level_count});
+  const PbsParams p{lwe_dimension, glwe_dimension, polynomial_size, base_log,
+                    level_count, std::max(grouping_factor, 1u)};
+  pbs_scratch(buffer, p.type(), "OPRF", p);
   if (num_blocks == 0)
     return;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -2131,9 +2182,7 @@ void b200_grouped_oprf_64_async(
   launch_pbs(st, gpu_index, static_cast<uint64_t *>(lwe_out), idx,
              static_cast<const uint64_t *>(lut_vector),
              static_cast<const uint64_t *>(lut_indexes), ws, idx,
-             bootstrapping_key, lwe_dimension, glwe_dimension, polynomial_size,
-             base_log, level_count, multi_bit ? grouping_factor : 1, num_blocks,
-             1, 0, 0);
+             bootstrapping_key, p, num_blocks, 1, 0, 0);
   const uint64_t big_n = (uint64_t)glwe_dimension * polynomial_size;
   launch(oprf_add_corrections_kernel,
          {(num_blocks + 255) / 256, 256, 0, st, gpu_index},
@@ -2167,14 +2216,12 @@ void b200_expand_without_verification_64_async(
     uint32_t pbs_base_log, uint32_t pbs_level_count, uint32_t grouping_factor) {
   set_device(gpu_index);
   check_polynomial_size(polynomial_size);
-  const bool multi_bit = grouping_factor > 1;
+  const PbsParams p{lwe_dimension, glwe_dimension, polynomial_size,
+                    pbs_base_log, pbs_level_count, std::max(grouping_factor, 1u)};
   const uint64_t T = compact_lists_total(num_lwes_per_compact_list,
                                          num_compact_lists,
                                          compact_lwe_dimension);
-  const PbsScratch &s =
-      pbs_scratch(buffer, multi_bit ? MULTI_BIT : CLASSICAL, "expand",
-                  PbsShape{glwe_dimension, polynomial_size, pbs_level_count},
-                  2 * T);
+  const PbsScratch &s = pbs_scratch(buffer, p.type(), "expand", p, 2 * T);
   B200_PANIC_IF_FALSE(casting_ksk && (!casting_to_big || computing_ksk),
                       "Cuda error (expand): missing keyswitching key");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -2216,9 +2263,7 @@ void b200_expand_without_verification_64_async(
   launch_pbs(st, gpu_index, static_cast<uint64_t *>(lwe_array_out), out_idx,
              static_cast<const uint64_t *>(lut_vector),
              static_cast<const uint64_t *>(lut_indexes), small, in_idx,
-             bootstrapping_key, lwe_dimension, glwe_dimension, polynomial_size,
-             pbs_base_log, pbs_level_count, multi_bit ? grouping_factor : 1,
-             samples, 1, 0, s.centered_ms);
+             bootstrapping_key, p, samples, 1, 0, s.centered_ms);
   B200_CHECK(cudaFreeAsync(ws, st));
 }
 
@@ -2392,10 +2437,10 @@ void b200_decompress_lwe_ciphertexts_64_async(
   check_compression_layout(lwe_per_glwe, compression_polynomial_size,
                            storage_log_modulus);
   check_polynomial_size(polynomial_size);
-  const bool multi_bit = grouping_factor > 1;
-  pbs_scratch(buffer, multi_bit ? MULTI_BIT : CLASSICAL, "decompression",
-              PbsShape{glwe_dimension, polynomial_size, level_count},
-              num_indexes);
+  const uint32_t big_n = compression_glwe_dimension * compression_polynomial_size;
+  const PbsParams p{big_n, glwe_dimension, polynomial_size, base_log,
+                    level_count, std::max(grouping_factor, 1u)};
+  pbs_scratch(buffer, p.type(), "decompression", p, num_indexes);
   if (num_indexes == 0)
     return;
   // trivial PBS indexes, one all-zero LUT index per sample, then the list
@@ -2410,7 +2455,6 @@ void b200_decompress_lwe_ciphertexts_64_async(
     h_idx[2 * (size_t)num_indexes + r] = indexes[r];
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const uint32_t big_n = compression_glwe_dimension * compression_polynomial_size;
   const uint64_t lwe_words = (uint64_t)num_indexes * (big_n + 1);
   uint64_t *ws = nullptr;
   B200_CHECK(cudaMallocFromPoolAsync(
@@ -2430,9 +2474,7 @@ void b200_decompress_lwe_ciphertexts_64_async(
   // 2^(64 - storage_log_modulus) and must not move (as in the grouped OPRF)
   launch_pbs(st, gpu_index, static_cast<uint64_t *>(lwe_out), iota,
              static_cast<const uint64_t *>(lut_vector), lut_idx, extracted, iota,
-             bootstrapping_key, big_n, glwe_dimension, polynomial_size,
-             base_log, level_count, multi_bit ? grouping_factor : 1,
-             num_indexes, 1, 0, 0);
+             bootstrapping_key, p, num_indexes, 1, 0, 0);
   B200_CHECK(cudaFreeAsync(ws, st));
 }
 
@@ -2448,10 +2490,10 @@ void b200_apply_noise_squashing_64_async(
   pbs128_instance(glwe_dimension, polynomial_size, pbs_level_count,
                   pbs_base_log);
   const uint32_t packed = (num_blocks + 1) / 2;
+  const PbsParams p{lwe_dimension, glwe_dimension, polynomial_size,
+                    pbs_base_log, pbs_level_count, 1};
   const PbsScratch &s =
-      pbs_scratch(buffer, CLASSICAL, "noise squashing",
-                  PbsShape{glwe_dimension, polynomial_size, pbs_level_count},
-                  packed, true);
+      pbs_scratch(buffer, p.type(), "noise squashing", p, packed, true);
   if (num_blocks == 0)
     return;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -2692,7 +2734,8 @@ void b200_bit_circuit_64_async(
                       "Cuda error (bit circuit): big LWE dimension %u is not "
                       "k * N = %u", big_lwe_dimension,
                       glwe_dimension * polynomial_size);
-  const bool multi_bit = grouping_factor > 1;
+  const PbsParams p{lwe_dimension, glwe_dimension, polynomial_size,
+                    pbs_base_log, pbs_level_count, std::max(grouping_factor, 1u)};
   // output rows of every layer, and the widest
   std::vector<uint64_t> outs(num_layers);
   uint64_t widest = 0;
@@ -2704,9 +2747,7 @@ void b200_bit_circuit_64_async(
                               layer_shared_rows[L], num_instances);
     widest = std::max(widest, outs[L]);
   }
-  const PbsScratch &s = pbs_scratch(
-      buffer, multi_bit ? MULTI_BIT : CLASSICAL, "bit circuit",
-      PbsShape{glwe_dimension, polynomial_size, pbs_level_count}, widest);
+  const PbsScratch &s = pbs_scratch(buffer, p.type(), "bit circuit", p, widest);
   if (widest == 0)
     return;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -2739,10 +2780,8 @@ void b200_bit_circuit_64_async(
     launch_pbs(st, gpu_index, d_pool, out_idx + out_base,
                static_cast<const uint64_t *>(lut_vector), lut_idx + out_base,
                small, static_cast<const uint64_t *>(input_indexes),
-               bootstrapping_key, lwe_dimension, glwe_dimension,
-               polynomial_size, pbs_base_log, pbs_level_count,
-               multi_bit ? grouping_factor : 1, (uint32_t)outs[L], 1, 0,
-               multi_bit ? 0 : s.centered_ms);
+               bootstrapping_key, p, (uint32_t)outs[L], 1, 0,
+               p.grouping > 1 ? 0 : s.centered_ms);
     out_base += outs[L];
   }
   B200_CHECK(cudaFreeAsync(ws, st));
@@ -2758,8 +2797,8 @@ const char *b200_last_keyswitch_kernel(void) { return t_last_ks_kernel; }
 
 int b200_pbs_uses_fast_path(uint32_t lwe_dimension, uint32_t glwe_dimension,
                             uint32_t polynomial_size, uint32_t level_count) {
-  return uses_fast_path(lwe_dimension, glwe_dimension, polynomial_size,
-                        level_count);
+  return pbs_route(PbsParams{lwe_dimension, glwe_dimension, polynomial_size, 0,
+                             level_count, 1}) == PbsRoute::N2048;
 }
 
 const char *b200_version(void) { return "tfhe-rs_b200 0.1 (sm_90a)"; }
