@@ -321,8 +321,8 @@ class CudaBooleanBlock:
 class CudaRadixServerKey:
     """Mirror of integer::gpu::CudaServerKey: the multiplication path
     (integer/gpu/server_key/radix/mul.rs:167), and comparisons, selects,
-    additions, subtractions, bitwise operations and erc7984's transfer,
-    compiled to KS -> PBS layers (`radix`) and run by a bit-circuit runner of
+    additions, subtractions, bitwise operations, erc7984's transfer
+    (`radix`) and divisions (`radix_div`), compiled to KS -> PBS layers and run by a bit-circuit runner of
     its own (created on first use) with `b200_bit_circuit_64_async`.
 
     Those operations take ciphertexts of one kind (unsigned or signed), one
@@ -385,14 +385,19 @@ class CudaRadixServerKey:
     def _run(self, op, signed, n, I, blocks, iconsts=None):
         """the circuit of (op, n, signed) on the operands' blocks, concatenated
         per instance; returns the outputs [I, outputs, big + 1]"""
-        import torch
-
         from . import radix
+
+        return self._run_circuit(radix.circuit(op, n, signed), I, blocks, iconsts)
+
+    def _run_circuit(self, circuit, I, blocks, iconsts=None):
+        """`circuit` on the operands' blocks, concatenated per instance;
+        returns the outputs [I, outputs, big + 1]"""
+        import torch
 
         W = blocks[0].shape[1]
         parts = [b.reshape(I, -1, W) for b in blocks]
         inst = parts[0] if len(parts) == 1 else torch.cat(parts, 1)
-        return self.runner.run(radix.circuit(op, n, signed), None, inst.reshape(-1, W), iconsts, I).view(I, -1, W)
+        return self.runner.run(circuit, None, inst.reshape(-1, W), iconsts, I).view(I, -1, W)
 
     @staticmethod
     def _radix(kind, out, I):
@@ -525,3 +530,57 @@ class CudaRadixServerKey:
             raise ValueError("transfer takes unsigned integers")
         out = self._run("transfer", False, n, I, [from_amount.blocks, to_amount.blocks, amount.blocks])
         return self._radix(kind, out[:, :n], I), self._radix(kind, out[:, n:], I)
+
+    # -- division (`radix_div`) --------------------------------------------------
+    def _div(self, op, lhs, rhs):
+        from . import radix_div
+
+        kind, n, I = self._operands(lhs, rhs)
+        out = self._run_circuit(radix_div.circuit(op, n, kind.signed), I, [lhs.blocks, rhs.blocks])
+        return self._div_results(op, kind, n, I, out)
+
+    def _scalar_div(self, op, lhs, scalar):
+        """`scalar` is one clear divisor for every input, or one per input"""
+        from . import radix_div
+
+        kind, n, I = self._operands(lhs)
+        scalars = [scalar] * I if np.ndim(scalar) == 0 else list(scalar)
+        if len(scalars) != I:
+            raise ValueError(f"expected one scalar or {I}, got {len(scalars)}")
+        iconsts = radix_div.scalar_iconsts(scalars, n, kind.signed)
+        out = self._run_circuit(radix_div.circuit(f"scalar_{op}", n, kind.signed), I, [lhs.blocks], iconsts)
+        return self._div_results(op, kind, n, I, out)
+
+    def _div_results(self, op, kind, n, I, out):
+        if op == "div_rem":
+            return self._radix(kind, out[:, :n], I), self._radix(kind, out[:, n:], I)
+        return self._radix(kind, out, I)
+
+    def div_rem(self, numerator, divisor):
+        """(quotient, remainder) of numerator / divisor, per input.  Unsigned:
+        n // d and n % d.  Signed: the quotient truncated toward zero (MIN / -1
+        wraps to MIN) and the remainder with the sign of the numerator.  By an
+        encrypted zero: unsigned, (2^bits - 1, n); signed, (-1 if n >= 0 else
+        1, n), as tfhe-rs computes."""
+        return self._div("div_rem", numerator, divisor)
+
+    def div(self, numerator, divisor):
+        """the quotient of `div_rem`"""
+        return self._div("div", numerator, divisor)
+
+    def rem(self, numerator, divisor):
+        """the remainder of `div_rem`"""
+        return self._div("rem", numerator, divisor)
+
+    def scalar_div_rem(self, numerator, divisor):
+        """`div_rem` by a clear divisor (one for every input, or one per input);
+        a zero divisor or one outside the integer's range raises ValueError"""
+        return self._scalar_div("div_rem", numerator, divisor)
+
+    def scalar_div(self, numerator, divisor):
+        """the quotient of `scalar_div_rem`"""
+        return self._scalar_div("div", numerator, divisor)
+
+    def scalar_rem(self, numerator, divisor):
+        """the remainder of `scalar_div_rem`"""
+        return self._scalar_div("rem", numerator, divisor)
