@@ -322,8 +322,8 @@ class CudaRadixServerKey:
     """Mirror of integer::gpu::CudaServerKey: the multiplication path
     (integer/gpu/server_key/radix/mul.rs:167), and comparisons, selects,
     additions, subtractions, bitwise operations, erc7984's transfer
-    (`radix`) and divisions (`radix_div`), compiled to KS -> PBS layers and run by a bit-circuit runner of
-    its own (created on first use) with `b200_bit_circuit_64_async`.
+    (`radix`), divisions (`radix_div`) and shifts, rotations and bit counts (`radix_bits`), compiled to KS -> PBS
+    layers and run by a bit-circuit runner of its own (created on first use) with `b200_bit_circuit_64_async`.
 
     Those operations take ciphertexts of one kind (unsigned or signed), one
     block count and one `num_inputs`, on 2_2 keys, and raise ValueError before
@@ -584,3 +584,105 @@ class CudaRadixServerKey:
     def scalar_rem(self, numerator, divisor):
         """the remainder of `scalar_div_rem`"""
         return self._scalar_div("rem", numerator, divisor)
+
+    # -- shifts, rotations and bit counts (`radix_bits`) ------------------------
+    def _shift(self, op, ct, amount):
+        from . import radix_bits
+
+        kind, n, I = self._operands(ct)
+        if not isinstance(amount, CudaUnsignedRadixCiphertext) or amount.signed:
+            raise ValueError(f"the amount of {op} must be a CudaUnsignedRadixCiphertext, got {type(amount).__name__}")
+        _, amount_blocks, amount_inputs = self._operands(amount)
+        if amount_inputs != I:
+            raise ValueError(f"the amount holds {amount_inputs} input(s), the integer {I}")
+        out = self._run_circuit(radix_bits.circuit(op, n, kind.signed, amount_blocks), I, [ct.blocks, amount.blocks])
+        return self._radix(kind, out, I)
+
+    def _scalar_shift(self, op, ct, amount):
+        from . import radix_bits
+
+        kind, n, I = self._operands(ct)
+        circuit = radix_bits.circuit(f"scalar_{op}", n, kind.signed, amount)
+        return self._radix(kind, self._run_circuit(circuit, I, [ct.blocks]), I)
+
+    def _count(self, op, ct):
+        from . import radix_bits
+
+        kind, n, I = self._operands(ct)
+        out = self._run_circuit(radix_bits.circuit(op, n, kind.signed), I, [ct.blocks])
+        w = radix_bits.result_blocks(op, n)
+        count = self._radix(CudaUnsignedRadixCiphertext, out[:, :w], I)
+        return (count, CudaBooleanBlock(out[:, w], I)) if op == "checked_ilog2" else count
+
+    def left_shift(self, ct, amount):
+        """ct << amount per input, `amount` an unsigned radix ciphertext of any
+        block count in [1, 64]; 0 when amount >= 2 * num_blocks"""
+        return self._shift("left_shift", ct, amount)
+
+    def right_shift(self, ct, amount):
+        """ct >> amount per input (arithmetic for a signed ct); when amount >=
+        2 * num_blocks, 0, or -1 for a negative signed ct"""
+        return self._shift("right_shift", ct, amount)
+
+    def rotate_left(self, ct, amount):
+        """ct rotated left by (amount mod 2^m) mod bits, bits = 2 * num_blocks
+        and m = floor(log2 bits) + [bits is not a power of 2]: the amount bits
+        tfhe-rs' barrel shifter reads"""
+        return self._shift("rotate_left", ct, amount)
+
+    def rotate_right(self, ct, amount):
+        """ct rotated right, the amount read as in `rotate_left`"""
+        return self._shift("rotate_right", ct, amount)
+
+    def scalar_left_shift(self, ct, amount):
+        """ct << amount, `amount` a clear non-negative int for every input"""
+        return self._scalar_shift("left_shift", ct, amount)
+
+    def scalar_right_shift(self, ct, amount):
+        """ct >> amount (arithmetic for a signed ct), `amount` a clear
+        non-negative int for every input"""
+        return self._scalar_shift("right_shift", ct, amount)
+
+    def scalar_rotate_left(self, ct, amount):
+        """ct rotated left by amount mod 2 * num_blocks"""
+        return self._scalar_shift("rotate_left", ct, amount)
+
+    def scalar_rotate_right(self, ct, amount):
+        """ct rotated right by amount mod 2 * num_blocks"""
+        return self._scalar_shift("rotate_right", ct, amount)
+
+    def leading_zeros(self, ct):
+        """the leading zero bits of ct's bit pattern (signed integers too), an
+        unsigned integer of ceil((floor(log2 bits) + 1) / 2) blocks"""
+        return self._count("leading_zeros", ct)
+
+    def leading_ones(self, ct):
+        """the leading one bits of ct's bit pattern, as `leading_zeros`"""
+        return self._count("leading_ones", ct)
+
+    def trailing_zeros(self, ct):
+        """the trailing zero bits of ct's bit pattern, as `leading_zeros`"""
+        return self._count("trailing_zeros", ct)
+
+    def trailing_ones(self, ct):
+        """the trailing one bits of ct's bit pattern, as `leading_zeros`"""
+        return self._count("trailing_ones", ct)
+
+    def count_ones(self, ct):
+        """the one bits of ct's bit pattern, an unsigned integer of 16 blocks"""
+        return self._count("count_ones", ct)
+
+    def count_zeros(self, ct):
+        """the zero bits of ct's bit pattern, an unsigned integer of 16 blocks"""
+        return self._count("count_zeros", ct)
+
+    def ilog2(self, ct):
+        """floor(log2) of ct's bit pattern (a signed integer is read as its bit
+        pattern, as tfhe-rs does): (bits - 1) - leading_zeros, an unsigned
+        integer of ceil((floor(log2(bits - 1)) + 2) / 2) blocks; all ones for 0"""
+        return self._count("ilog2", ct)
+
+    def checked_ilog2(self, ct):
+        """(`ilog2`, ct > 0): the flag compares with ct's own signedness, as
+        tfhe-rs does, so it is 0 for a negative signed ct"""
+        return self._count("checked_ilog2", ct)
