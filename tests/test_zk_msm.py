@@ -5,7 +5,11 @@ CPU: the header's constants, field and group law through its g++ build
 (tests/emu/zk_host.cpp), the window digits, the ABI struct layout, the
 exported symbols, the host-only C wrappers and argument checking.
 GPU: G1 and G2 MSMs word for word against the model, edge batches, the managed
-and unmanaged calls, and parity with the reference's zk library when built."""
+and unmanaged calls, and parity with the reference's zk library when built;
+one MSM at and just below the smallest n of every window size, buckets at the
+task and tree-pass edges, and the unmanaged call on a scratch of exactly the
+reported size.  tests/test_zk_device_arith.py checks the device field and
+curve code op by op."""
 import ctypes as C
 import os
 import random
@@ -467,3 +471,145 @@ def test_parity_with_the_reference_library(name, n):
         results.append(out)
     assert results[0].tobytes() == results[1].tobytes()
     assert zk.normalized_to_affine(g, results[0]) == M.msm_by_logs(curve, [zk.limbs_to_int(k) for k in ks], logs)
+
+
+# ---------------------------------------------------- every window plan ---
+# msm_plan picks c in [4, 16] for G1 and [4, 14] for G2 minimising
+# num_windows(c) (n + 3 2^(c-1)); the smallest n of each c:
+PLAN_THRESHOLDS = {4: 1, 5: 74, 6: 188, 7: 457, 8: 1383, 9: 2381, 10: 7681, 11: 13825, 12: 24577, 13: 70657,
+                   14: 129025, 15: 516097, 16: 983041}
+C_MAX = {"g1": 16, "g2": 14}
+POOL = 2048  # points are drawn cyclically from this many known multiples
+
+
+def _plan_c(n, cmax):
+    best = pc = None
+    for c in range(4, cmax + 1):
+        cost = (320 // c + 1) * (n + 3 * (1 << (c - 1)))
+        if best is None or cost < best:
+            best, pc = cost, c
+    return pc
+
+
+def test_plan_thresholds_follow_the_cost_formula():
+    for name, cmax in C_MAX.items():
+        for c in range(4, cmax + 1):
+            n = PLAN_THRESHOLDS[c]
+            assert _plan_c(n, cmax) == c and (n == 1 or _plan_c(n - 1, cmax) == c - 1), (name, c)
+    assert _plan_c(1 << 31, 14) == 14 and _plan_c(1 << 31, 16) == 16
+
+
+PLAN_ROWS = [(name, n) for name, cmax in C_MAX.items() for c in range(4, cmax + 1)
+             for n in sorted({PLAN_THRESHOLDS[c], PLAN_THRESHOLDS[c] - 1} - {0})]
+SEEN_C = {"g1": set(), "g2": set()}
+COMPLETED_PLANS = set()
+
+
+def _pool(name):
+    """(curve, logs, normal-form ABI pool, Montgomery ABI pool) of POOL points"""
+    _, g, logs, _, normal, montp = _batch(name, POOL, seed=23)
+    return (M.G1 if name == "g1" else M.G2), g, logs, normal, montp
+
+
+def _cyclic(name, n, seed):
+    """n points P_i = pool[i mod POOL], n random 320-bit scalars, and the
+    model's sum k_i log(i mod POOL) G"""
+    curve, g, logs, normal, montp = _pool(name)
+    idx = np.arange(n) % POOL
+    ks = np.random.default_rng(seed).integers(0, 1 << 64, size=(n, 5), dtype=np.uint64)
+    # per pool point, the sum of its scalars: 32-bit halves summed exactly in
+    # float64 (at most 481 terms below 2^32 each)
+    halves = ks.view(np.uint32).reshape(n, 10)
+    sums = [np.bincount(idx, weights=halves[:, h], minlength=POOL) for h in range(10)]
+    e = sum(logs[j] * sum(int(sums[h][j]) << (32 * h) for h in range(10)) for j in range(POOL)) % M.R_ORDER
+    return normal[idx], montp[idx], ks, curve.mul(e, curve.gen)
+
+
+def _last_config():
+    from tfhe_rs_b200 import _lib
+
+    cfg = _lib.lib().b200_last_msm_config().decode()
+    return {k: int(v) for k, v in re.findall(r"\b(c|windows|task|segments)=(\d+)", cfg)}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,n", PLAN_ROWS)
+def test_msm_at_every_window_plan(name, n):
+    """One MSM at the smallest n of each window size c, and at one less; the
+    plan that ran is read back from b200_last_msm_config()."""
+    c = _plan_c(n, C_MAX[name])
+    normal, _, ks, expect = _cyclic(name, n, seed=n)
+    assert _gpu_msm(name, normal, ks) == expect
+    cfg = _last_config()
+    assert cfg["c"] == c and cfg["windows"] == 320 // c + 1, cfg
+    assert cfg["segments"] == min(1 << (c - 1), 64) and cfg["task"] == 8, cfg
+    SEEN_C[name].add(c)
+    COMPLETED_PLANS.add((name, n))
+
+
+@pytest.mark.gpu
+def test_window_plans_cover_every_c():
+    """Runs after the plan table (same module): every c of each group ran."""
+    if len(COMPLETED_PLANS) < len(PLAN_ROWS):
+        pytest.skip("the plan table did not run in this session")
+    assert SEEN_C == {"g1": set(range(4, 17)), "g2": set(range(4, 15))}, SEEN_C
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,c", [(name, c) for name, cmax in C_MAX.items() for c in range(4, cmax + 1)])
+def test_unmanaged_scratch_of_exactly_the_reported_size(name, c):
+    """A scratch of exactly pippenger_scratch_size bytes, filled with a
+    sentinel and followed by a sentinel guard: the result matches the model
+    and the guard is untouched."""
+    import torch
+
+    from tfhe_rs_b200 import gpu, zk
+
+    n = PLAN_THRESHOLDS[c]
+    _, montp, ks, expect = _cyclic(name, n, seed=1000 + n)
+    g = zk.G1 if name == "g1" else zk.G2
+    streams = gpu.CudaStreams.new_single_gpu(0)
+    need = zk.scratch_size(g, n)
+    guard = 1 << 16
+    buf = torch.full((need + guard,), 0xA5, dtype=torch.uint8, device=streams.device(0))
+    torch.cuda.synchronize()
+    raw = zk.msm_device(g, zk.to_device(montp, streams), zk.to_device(ks, streams), streams, scratch=buf[:need])
+    assert _last_config()["c"] == c
+    assert zk.normalized_to_affine(g, zk.normalize(g, raw)) == expect
+    torch.cuda.synchronize()
+    assert bool((buf[need:] == 0xA5).all()), "the MSM wrote past pippenger_scratch_size"
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", ["g1", "g2"])
+@pytest.mark.parametrize("n", [7, 8, 9, 15, 16, 17, 63, 64, 65, 129])
+def test_equal_scalars_at_task_and_tree_edges(name, n):
+    """Every scalar equal: each window's digit puts all n points in one bucket,
+    ceil(n / 8) tasks and log2 of that many tree passes."""
+    from tfhe_rs_b200 import zk
+
+    curve, g, logs, _, normal, _ = _batch(name, n)
+    for k in ((1 << 299) + 12345, M.R_ORDER - 1, (1 << 320) - 1):
+        assert _gpu_msm(name, normal, zk.scalars([k] * n)) == M.msm_by_logs(curve, [k] * n, logs), k
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", ["g1", "g2"])
+@pytest.mark.parametrize("c,groups", [(4, 8), (6, 32)])
+def test_every_bucket_holds_nine_points(name, c, groups):
+    """n = 9 groups: group j's scalar has digit j + 1 in every full window, so
+    every non-empty bucket holds 9 points, two tasks each (8 + 1).  The task
+    count is then within 10% of the plan's max_tasks bound."""
+    from tfhe_rs_b200 import zk
+
+    n = 9 * groups
+    assert _plan_c(n, C_MAX[name]) == c
+    W, B = 320 // c + 1, 1 << (c - 1)
+    tasks = 2 * groups * (W - 1)
+    max_tasks = n * W // 8 + min(W * B, n * W) + 1
+    assert 0.9 * max_tasks < tasks <= max_tasks
+    curve, g, logs, _, normal, _ = _batch(name, n)
+    digit = [sum((j + 1) << (c * w) for w in range(W - 1)) for j in range(groups)]
+    ks = [digit[i // 9] for i in range(n)]
+    assert _gpu_msm(name, normal, zk.scalars(ks)) == M.msm_by_logs(curve, ks, logs)
+    assert _last_config()["c"] == c
