@@ -321,8 +321,9 @@ class CudaBooleanBlock:
 class CudaRadixServerKey:
     """Mirror of integer::gpu::CudaServerKey: the multiplication path
     (integer/gpu/server_key/radix/mul.rs:167), and comparisons, selects,
-    additions, subtractions, bitwise operations, erc7984's transfer
-    (`radix`), divisions (`radix_div`) and shifts, rotations and bit counts (`radix_bits`), compiled to KS -> PBS
+    additions, subtractions, bitwise operations, their clear-operand forms,
+    signed overflow flags, abs, erc7984's transfer (`radix`), products and
+    sums (`radix_mul`), divisions (`radix_div`) and shifts, rotations and bit counts (`radix_bits`), compiled to KS -> PBS
     layers and run by a bit-circuit runner of its own (created on first use) with `b200_bit_circuit_64_async`.
 
     Those operations take ciphertexts of one kind (unsigned or signed), one
@@ -411,16 +412,29 @@ class CudaRadixServerKey:
         _, I, out = self._binary(op, lhs, rhs)
         return CudaBooleanBlock(out[:, 0], I)
 
-    def _scalar_compare(self, op, lhs, scalar) -> CudaBooleanBlock:
-        """`scalar` is one clear integer for every input, or one per input"""
+    def _scalar_iconsts(self, ct, scalar):
+        """(kind, n, I, iconsts) of a clear operand: `scalar` is one clear
+        integer for every input, or one per input"""
         from . import radix
 
-        kind, n, I = self._operands(lhs)
+        kind, n, I = self._operands(ct)
         scalars = [scalar] * I if np.ndim(scalar) == 0 else list(scalar)
         if len(scalars) != I:
             raise ValueError(f"expected one scalar or {I}, got {len(scalars)}")
-        iconsts = radix.scalar_iconsts(scalars, n, kind.signed)
+        return kind, n, I, radix.scalar_iconsts(scalars, n, kind.signed)
+
+    def _scalar_compare(self, op, lhs, scalar) -> CudaBooleanBlock:
+        """`scalar` is one clear integer for every input, or one per input"""
+        kind, n, I, iconsts = self._scalar_iconsts(lhs, scalar)
         return CudaBooleanBlock(self._run(f"scalar_{op}", kind.signed, n, I, [lhs.blocks], iconsts)[:, 0], I)
+
+    def _scalar_arith(self, op, ct, scalar):
+        """the blocks of op with a clear rhs, then its flag if it has one"""
+        kind, n, I, iconsts = self._scalar_iconsts(ct, scalar)
+        out = self._run(f"scalar_{op}", kind.signed, n, I, [ct.blocks], iconsts)
+        if out.shape[1] == n:
+            return self._radix(kind, out, I)
+        return self._radix(kind, out[:, :n], I), CudaBooleanBlock(out[:, n], I)
 
     def eq(self, lhs, rhs):
         return self._compare("eq", lhs, rhs)
@@ -505,6 +519,62 @@ class CudaRadixServerKey:
         """(lhs - rhs wrapping, [lhs < rhs])"""
         return self._overflowing("overflowing_sub", lhs, rhs)
 
+    def _signed_overflowing(self, op, lhs, rhs):
+        kind, n, I = self._operands(lhs, rhs)
+        if not kind.signed:
+            raise ValueError(f"signed_{op} takes signed integers")
+        out = self._run(f"signed_{op}", True, n, I, [lhs.blocks, rhs.blocks])
+        return self._radix(kind, out[:, :n], I), CudaBooleanBlock(out[:, n], I)
+
+    def signed_overflowing_add(self, lhs, rhs):
+        """(lhs + rhs wrapping, [the exact lhs + rhs is outside [MIN, MAX]])
+        for signed integers"""
+        return self._signed_overflowing("overflowing_add", lhs, rhs)
+
+    def signed_overflowing_sub(self, lhs, rhs):
+        """(lhs - rhs wrapping, [the exact lhs - rhs is outside [MIN, MAX]])
+        for signed integers"""
+        return self._signed_overflowing("overflowing_sub", lhs, rhs)
+
+    def scalar_add(self, ct, scalar):
+        """ct + scalar, wrapping mod 4^num_blocks; `scalar` is one clear
+        integer for every input, or one per input, in the integer's range
+        (else ValueError)"""
+        return self._scalar_arith("add", ct, scalar)
+
+    def scalar_sub(self, ct, scalar):
+        """ct - scalar, wrapping mod 4^num_blocks, `scalar` as in `scalar_add`"""
+        return self._scalar_arith("sub", ct, scalar)
+
+    def unsigned_overflowing_scalar_add(self, ct, scalar):
+        """(ct + scalar wrapping, [ct + scalar >= 4^num_blocks]) for an
+        unsigned ct, `scalar` as in `scalar_add`"""
+        if not isinstance(ct, CudaUnsignedRadixCiphertext) or ct.signed:
+            raise ValueError("unsigned_overflowing_scalar_add takes an unsigned integer")
+        return self._scalar_arith("overflowing_add", ct, scalar)
+
+    def signed_overflowing_scalar_add(self, ct, scalar):
+        """(ct + scalar wrapping, [the exact sum is outside [MIN, MAX]]) for a
+        signed ct, `scalar` as in `scalar_add`"""
+        if not isinstance(ct, CudaSignedRadixCiphertext):
+            raise ValueError("signed_overflowing_scalar_add takes a signed integer")
+        return self._scalar_arith("signed_overflowing_add", ct, scalar)
+
+    def signed_overflowing_scalar_sub(self, ct, scalar):
+        """(ct - scalar wrapping, [the exact difference is outside [MIN,
+        MAX]]) for a signed ct, `scalar` as in `scalar_add`"""
+        if not isinstance(ct, CudaSignedRadixCiphertext):
+            raise ValueError("signed_overflowing_scalar_sub takes a signed integer")
+        return self._scalar_arith("signed_overflowing_sub", ct, scalar)
+
+    def abs(self, ct):
+        """|ct| wrapping (abs(MIN) is MIN) for a signed ct; an unsigned ct comes
+        back as a copy (on the caller's current stream), with no bootstrap"""
+        kind, n, I = self._operands(ct)
+        if not kind.signed:
+            return kind(ct.blocks.clone(), I)
+        return self._radix(kind, self._run("abs", True, n, I, [ct.blocks]), I)
+
     def bitand(self, lhs, rhs):
         kind, I, out = self._binary("bitand", lhs, rhs)
         return self._radix(kind, out, I)
@@ -521,6 +591,18 @@ class CudaRadixServerKey:
         kind, n, I = self._operands(ct)
         return self._radix(kind, self._run("bitnot", False, n, I, [ct.blocks]), I)
 
+    def scalar_bitand(self, ct, scalar):
+        """ct & scalar on the two's-complement bits, `scalar` as in `scalar_add`"""
+        return self._scalar_arith("bitand", ct, scalar)
+
+    def scalar_bitor(self, ct, scalar):
+        """ct | scalar on the two's-complement bits, `scalar` as in `scalar_add`"""
+        return self._scalar_arith("bitor", ct, scalar)
+
+    def scalar_bitxor(self, ct, scalar):
+        """ct ^ scalar on the two's-complement bits, `scalar` as in `scalar_add`"""
+        return self._scalar_arith("bitxor", ct, scalar)
+
     def transfer(self, from_amount, to_amount, amount):
         """erc7984's `transfer_whitepaper` on unsigned balances, in one
         circuit: sent = amount if from_amount >= amount else 0; returns
@@ -530,6 +612,58 @@ class CudaRadixServerKey:
             raise ValueError("transfer takes unsigned integers")
         out = self._run("transfer", False, n, I, [from_amount.blocks, to_amount.blocks, amount.blocks])
         return self._radix(kind, out[:, :n], I), self._radix(kind, out[:, n:], I)
+
+    # -- products and sums (`radix_mul`) ---------------------------------------
+    def mul(self, lhs, rhs):
+        """lhs * rhs wrapping mod 4^num_blocks, per input (the low half of the
+        product, the same bits for signed and unsigned integers)"""
+        from . import radix_mul
+
+        kind, n, I = self._operands(lhs, rhs)
+        return self._radix(kind, self._run_circuit(radix_mul.circuit("mul", n), I, [lhs.blocks, rhs.blocks]), I)
+
+    def scalar_mul(self, ct, scalar):
+        """ct * scalar wrapping mod 4^num_blocks; `scalar` is one clear integer
+        for every input, or one per input, in the integer's range (else
+        ValueError)"""
+        from . import radix_mul
+
+        kind, n, I, iconsts = self._scalar_iconsts(ct, scalar)
+        return self._radix(kind, self._run_circuit(radix_mul.circuit("scalar_mul", n), I, [ct.blocks], iconsts), I)
+
+    def unsigned_overflowing_mul(self, lhs, rhs):
+        """(lhs * rhs wrapping, [lhs * rhs >= 4^num_blocks]) for unsigned
+        integers"""
+        from . import radix_mul
+
+        kind, n, I = self._operands(lhs, rhs)
+        if kind.signed:
+            raise ValueError("unsigned_overflowing_mul takes unsigned integers")
+        out = self._run_circuit(radix_mul.circuit("unsigned_overflowing_mul", n), I, [lhs.blocks, rhs.blocks])
+        return self._radix(kind, out[:, :n], I), CudaBooleanBlock(out[:, n], I)
+
+    def signed_overflowing_mul(self, lhs, rhs):
+        """(lhs * rhs wrapping, [the exact lhs * rhs is outside [MIN, MAX]])
+        for signed integers"""
+        from . import radix_mul
+
+        kind, n, I = self._operands(lhs, rhs)
+        if not kind.signed:
+            raise ValueError("signed_overflowing_mul takes signed integers")
+        out = self._run_circuit(radix_mul.circuit("signed_overflowing_mul", n), I, [lhs.blocks, rhs.blocks])
+        return self._radix(kind, out[:, :n], I), CudaBooleanBlock(out[:, n], I)
+
+    def sum_ciphertexts(self, cts):
+        """the wrapping sum of a list of integers of one kind, block count and
+        num_inputs, per input; None for an empty list (tfhe-rs' Option)"""
+        from . import radix_mul
+
+        cts = list(cts)
+        if not cts:
+            return None
+        kind, n, I = self._operands(*cts)
+        out = self._run_circuit(radix_mul.circuit("sum", n, len(cts)), I, [ct.blocks for ct in cts])
+        return self._radix(kind, out, I)
 
     # -- division (`radix_div`) --------------------------------------------------
     def _div(self, op, lhs, rhs):

@@ -30,7 +30,11 @@ per-instance body constants).  Circuits:
     (sub: a + 3 - b, + 1 into block 0), a Hillis-Steele scan of the states
     with `integer`'s combine table on 4 cur + prev, and one PBS per block on
     m_i + 4 state_{i-1} (noise 5, value <= 11); the carry out is folded into
-    the scan's last combine of the top block.
+    the scan's last combine of the top block;
+  * signed overflow of add / sub: one PBS on 4 a_top + b_top (sub: 3 - b_top)
+    gives a code {never, iff carry, iff no carry, always}, and one PBS on
+    4 code + state_{n-2}, beside the last layer, the flag;
+  * abs: `radix_div.cond_negate` on the sign block.
 """
 from __future__ import annotations
 
@@ -58,9 +62,18 @@ ORDER_FINAL = {"gt": lambda s: s == SUPERIOR, "ge": lambda s: s != INFERIOR,
                "lt": lambda s: s == INFERIOR, "le": lambda s: s != SUPERIOR}
 BITOPS = {"bitand": lambda l, r: l & r, "bitor": lambda l, r: l | r, "bitxor": lambda l, r: l ^ r}
 # operations whose circuit depends on the signedness of the operands
-SIGNED_OPS = ("gt", "ge", "lt", "le", "min", "max") + tuple(f"scalar_{o}" for o in ("gt", "ge", "lt", "le"))
+SIGNED_OPS = ("gt", "ge", "lt", "le", "min", "max", "abs") + tuple(f"scalar_{o}" for o in ("gt", "ge", "lt", "le"))
+# additions with a flag: (flag, signed flag) by base operation
+ADDS = {"add": (False, False), "sub": (False, False), "overflowing_add": (True, False),
+        "overflowing_sub": (True, False), "signed_overflowing_add": (True, True),
+        "signed_overflowing_sub": (True, True)}
 OPERATIONS = (COMPARISONS + tuple(f"scalar_{o}" for o in COMPARISONS) + ("min", "max", "if_then_else", "add",
               "sub", "neg", "overflowing_add", "overflowing_sub", "bitnot", "transfer") + tuple(BITOPS))
+# clear-operand arithmetic, signed overflow flags and abs: circuits of this
+# module too, kept apart from OPERATIONS, whose every schedule is pinned as is
+ARITH_OPERATIONS = (("signed_overflowing_add", "signed_overflowing_sub", "abs")
+                    + tuple(f"scalar_{o}" for o in ("add", "sub", "overflowing_add", "signed_overflowing_add",
+                                                    "signed_overflowing_sub") + tuple(BITOPS)))
 
 Block = List[Tuple[int, int]]   # (wire, coef) terms of one operand block's value
 
@@ -179,12 +192,20 @@ def if_then_else(c: bc.Circuit, cond: int, a: Sequence[Block], b: Sequence[Block
 # ---------------------------------------------------------------------------
 # additions
 # ---------------------------------------------------------------------------
+def _signed_overflow(top: int, carry: int) -> bool:
+    """whether a signed sum leaves [MIN, MAX], from 4 a_top + b_top (b_top the
+    top digit of ~b for a subtraction) and the carry into the top block"""
+    t = _signed_digit(top // MSG_MOD) + _signed_digit(top % MSG_MOD) + carry
+    return not -MSG_MOD // 2 <= t < MSG_MOD // 2
+
+
 def add(c: bc.Circuit, a: Optional[Sequence[Block]], b: Sequence[Block], sub: bool = False,
-        flag: bool = False) -> Tuple[List[int], Optional[int]]:
+        flag: bool = False, signed: bool = False) -> Tuple[List[int], Optional[int]]:
     """a + b, or a - b (a + ~b + 1; a None is 0: the negation of b), wrapping
     mod 4^blocks.  With `flag`, also the carry out of a + b, or for a - b the
-    borrow [a < b] (tfhe-rs' unsigned overflow flags).  Returns (blocks,
-    flag wire or None)."""
+    borrow [a < b] (tfhe-rs' unsigned overflow flags); with `flag` and
+    `signed`, [the exact two's-complement result is outside [MIN, MAX]].
+    Returns (blocks, flag wire or None)."""
     n = len(b)
     sums: List[Tuple[Block, int]] = []
     for i in range(n):
@@ -196,6 +217,17 @@ def add(c: bc.Circuit, a: Optional[Sequence[Block]], b: Sequence[Block], sub: bo
             sums.append((terms + list(b[i]), 0))
     flag_f = (lambda s: s != integer.ST_GENERATE) if sub else (lambda s: s == integer.ST_GENERATE)
     msgs = [_pbs(c, t, body, lambda v: MSG_TABLE[v]) for t, body in sums]
+    code = None
+    if flag and signed:
+        # 4 a_top + b_top (sub: 3 - b_top), noise 5: with the carry into the
+        # top block known (n == 1) the flag, else a code read with the carry
+        # state: 0 never, 1 iff carry, 2 iff no carry, 3 always
+        top = (_scaled(a[n - 1], MSG_MOD) + (_scaled(b[n - 1], -1) if sub else list(b[n - 1])),
+               MSG_MOD - 1 if sub else 0)
+        if n == 1:
+            return msgs, _pbs(c, *top, lambda v: int(_signed_overflow(v, int(sub))))
+        code = _pbs(c, *top, lambda v: int(_signed_overflow(v, 1)) + 2 * int(_signed_overflow(v, 0)))
+        flag = False
     if flag and n == 1:
         return msgs, _pbs(c, *sums[0], lambda v: flag_f(STATE_TABLE[v]))
     # inclusive prefix states of blocks 0..i: the state feeding block i + 1,
@@ -215,6 +247,9 @@ def add(c: bc.Circuit, a: Optional[Sequence[Block]], b: Sequence[Block], sub: bo
                               lambda v: COMBINE_TABLE[v] if v <= 10 else 0)
         states = nxt
         d *= 2
+    if code is not None:   # one PBS on 4 code + state_{n-2}, beside the last layer
+        out_flag = _pbs(c, [(code, MSG_MOD), (states[n - 2], 1)], 0,
+                        lambda v: (v // MSG_MOD >> int(v % MSG_MOD != integer.ST_GENERATE)) & 1)
     out = [msgs[0]] + [_pbs(c, [(msgs[i], 1), (states[i - 1], MSG_MOD)], 0,
                             lambda v: (v % MSG_MOD + CARRY_TABLE[v // MSG_MOD]) % MSG_MOD if v < 12 else 0)
                        for i in range(1, n)]
@@ -255,14 +290,15 @@ def circuit(op: str, num_blocks: int, signed: bool = False) -> bc.Circuit:
     """The circuit of one operation on `num_blocks`-block integers.  Per
     instance, inputs are the operands' blocks in argument order
     (`if_then_else`: the condition block first) and the outputs are the
-    result's blocks: a boolean is one block; `overflowing_*` output the
-    blocks then the flag; `transfer` new_from then new_to.  `scalar_*` read
-    the clear rhs as 2 * num_blocks per-instance bits (`scalar_iconsts`).
+    result's blocks: a boolean is one block; the `overflowing_*` operations
+    output the blocks then the flag; `transfer` new_from then new_to.
+    `scalar_*` read the clear rhs as 2 * num_blocks per-instance bits
+    (`scalar_iconsts`).  `op` is one of OPERATIONS or ARITH_OPERATIONS.
     The CIRCUIT_CACHE_SIZE most recent (op, num_blocks, signed) are kept (an
     operation that does not depend on the signedness has one circuit); the
     schedule of each is compiled once (`bit_circuit.schedule`)."""
     n = check_num_blocks(num_blocks)
-    if op not in OPERATIONS:
+    if op not in OPERATIONS + ARITH_OPERATIONS:
         raise ValueError(f"unknown radix operation {op!r}")
     return _circuit(op, n, bool(signed) and op in SIGNED_OPS)
 
@@ -280,6 +316,12 @@ def _circuit(op: str, n: int, signed: bool) -> bc.Circuit:
         new_from, new_to = transfer(c, frm, to, amount)
         c.output_blocks(new_from + new_to)
         return c
+    if op == "abs":   # unsigned: the identity
+        from . import radix_div
+
+        x = c.inputs_block(n, False)
+        c.output_blocks(radix_div.cond_negate(c, x, x[-1], lambda v: v >= MSG_MOD // 2) if signed else x)
+        return c
     a = blocks_of(c.inputs_block(n, False))
     if op in ("neg", "bitnot"):
         c.output_blocks(add(c, None, a, sub=True)[0] if op == "neg" else bitnot(c, a))
@@ -291,8 +333,8 @@ def _circuit(op: str, n: int, signed: bool) -> bc.Circuit:
     elif base in ("min", "max"):
         gt = compare(c, a, b, "gt", signed)
         c.output_blocks(if_then_else(c, gt, b, a) if base == "min" else if_then_else(c, gt, a, b))
-    elif base in ("add", "sub", "overflowing_add", "overflowing_sub"):
-        out, flag = add(c, a, b, sub=base.endswith("sub"), flag=base.startswith("overflowing"))
+    elif base in ADDS:
+        out, flag = add(c, a, b, sub=base.endswith("sub"), flag=ADDS[base][0], signed=ADDS[base][1])
         c.output_blocks(out + ([flag] if flag is not None else []))
     else:
         c.output_blocks(bitop(c, a, b, base))
