@@ -275,12 +275,16 @@ static const N2048Instance N2048_INSTANCES[] = {
     {18, pbs_n2048_k1_l1_v6_kernel<2, true, 3>, sizeof(P22SmemV6<2, true>), "n2048_v6<2,true,3>"},
     // the shipped one-CTA instance (see launch_pbs)
     {19, pbs_n2048_k1_l1_v6_kernel<0, true, 2>, sizeof(P22SmemV6<4, true>), "n2048_v6<0,true,2>"},
-    // the shipped two-CTA instance (lane-pair layout, see launch_pbs)
+    // the shipped two-CTA instance (lane-pair layout, exchange 2 through the
+    // warp's own rows of the exchange-1 buffer; see launch_pbs)
     {20, pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1>, sizeof(P22SmemV6<2, true>), "n2048_v6<2,true,2,1>"},
     {21, pbs_n2048_k1_l1_v6_kernel<0, true, 2, 1>, sizeof(P22SmemV6<4, true>), "n2048_v6<0,true,2,1>"},
     // v6 hybrid with both CTA barriers of a step split (own-row products before
     // the wait for the other group's spectrum)
     {22, pbs_n2048_k1_l1_v6_kernel<2, true, 2, 2>, sizeof(P22SmemV6<2, true>), "n2048_v6<2,true,2,2>"},
+    // the shipped two-CTA instance with exchange 2 through half-warp shuffles
+    // (x2_shfl.cuh), its A/B partner
+    {23, pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1, 0>, sizeof(P22SmemV6<2, true>), "n2048_v6<2,true,2,1,0>"},
 };
 static const N2048Instance *n2048_instance(int variant) {
   for (const N2048Instance &r : N2048_INSTANCES)
@@ -590,11 +594,12 @@ static void launch_n2048(cudaStream_t stream, uint32_t gpu_index,
     // registers, other row (the one v3 waited a full L2 round trip for)
     // through the ring; rotate + decompose with the sign as a predicate
     // (CVT = 2); lane-pair layout: each warp holds the same 16 threads of
-    // both polynomials (lanes l and l ^ 16), exchange 2 through half-warp
-    // shuffles, the other polynomial's spectrum taken with one shuffle in
-    // the MAC (no spectrum store, no barrier between the polynomials).
-    // Bit-identical to variant 17, the same instance in the 64-thread
-    // group layout.
+    // both polynomials (lanes l and l ^ 16), exchange 2 through the warp's
+    // own rows of the exchange-1 buffer (no shuffles, no selects), the other
+    // polynomial's spectrum taken with one shuffle in the MAC (no spectrum
+    // store, no barrier between the polynomials).  Bit-identical to variant
+    // 17, the same instance in the 64-thread group layout, and to variant 23,
+    // the same instance with exchange 2 through half-warp shuffles.
     variant = 20; // n2048_v6<2,true,2,1>
   }
   const N2048Instance &r = *n2048_instance(variant);

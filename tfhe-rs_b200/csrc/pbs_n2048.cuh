@@ -20,6 +20,7 @@
 #include "pbs_n2048_phases.cuh"
 #include "tma_bulk.cuh"
 #include "x2_shfl.cuh"
+#include "x2_smem.cuh"
 
 #include <cuda_runtime.h>
 
@@ -599,7 +600,9 @@ __device__ uint32_t g_p22_sm_arrivals[512];
 // (own row after the last forward pass, other row after the own products) --
 // the A/B partner that isolates the effect of the ring; 2: own row through
 // registers, other row (the one v3 waits for) through the ring.
-template <int KEY_MODE, bool STAGE_A, int CVT = 0, int SPLIT_POST = 0>
+// X2 (lane-pair layout only): exchange 2 through the warp's own rows of xa[g]
+// (1, x2m_*, x2_smem.cuh) or through half-warp shuffles (0, x2h_*).
+template <int KEY_MODE, bool STAGE_A, int CVT = 0, int SPLIT_POST = 0, int X2 = 1>
 __global__ void __launch_bounds__(128, 2)
 pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
                           const uint64_t *__restrict__ out_idx,
@@ -735,10 +738,13 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
     // polynomial l >> 4, so lanes l and l ^ 16 hold the same spectrum slots
     // 16 t + b of the two polynomials after the forward transform.  The MAC
     // takes the other polynomial's value with one shuffle: no spectrum store,
-    // no barrier between the polynomials before or after it.  Exchange 2 stays
-    // inside each half-warp (x2h_*), exchange 1 goes through xa[g] (x1h_*), and
-    // the values and the order of every operation are those of the other
-    // instances, so the results are bit-identical.
+    // no barrier between the polynomials before or after it.  Exchange 1 goes
+    // through xa[g] (x1h_*); exchange 2 goes through this warp's rows of the
+    // same buffer (X2 = 1, x2m_*: they belong to the warp from x1h_load_p2 to
+    // x1h_store_p2) or stays inside each half-warp as shuffles (X2 = 0,
+    // x2h_*).  The values and the order of every operation are those of the
+    // other instances, so the results are bit-identical.
+    [[maybe_unused]] cplx *x2_rows = xa_g + 256 * (tid >> 5);
     for (uint32_t i = 0; i < n; i++) {
       const uint32_t a = a_next; // read a step ahead: every address of the step hangs on it
       a_next = sm.a_hat[i + 1];  // a_hat has 8 words of padding
@@ -749,7 +755,10 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
       __syncthreads();
       x1h_load_p2(xa_g, t, v);
       pass2_fwd(v, tw2);
-      x2h_fwd(v);
+      if constexpr (X2 == 1)
+        x2m_fwd(x2_rows, v);
+      else
+        x2h_fwd(v);
       radix16_fwd(v, tw3);
       const size_t step = (size_t)i * (4 * P22_M);
       cplx b_own[16];
@@ -763,10 +772,14 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
         v[b] = cfma(o, k_oth[b * 64 + t], cmul(v[b], b_own[b]));
       }
       radix16_inv(v, tw3);
-      x2h_inv(v);
+      if constexpr (X2 == 1)
+        x2m_inv(x2_rows, v);
+      else
+        x2h_inv(v);
       pass2_inv(v, tw2);
-      // the forward exchange-1 loads of this warp read the same slots (rows
-      // 4 w .. 4 w + 3 of xa[g]); no other warp touches them in between
+      // the forward exchange-1 loads (or the exchange-2 loads) of this warp
+      // read the same slots (rows 4 w .. 4 w + 3 of xa[g]); no other warp
+      // touches them in between
       __syncwarp();
       x1h_store_p2(xa_g, t, v);
       __syncthreads();

@@ -1,9 +1,14 @@
 // tools/micro/phase_clocks.cu -- where do the cycles of ONE CMUX step go?
-// Replays the blind-rotation loop of pbs_n2048_k1_l1_v3_kernel (same phase
-// functions, same order) with a clock64() read between phases, for 1..2 CTAs
-// per SM, and prints the average cycles per phase of warp 0.  Measurement
-// tool only (not part of the library).
+// Replays the blind-rotation loop of the shipped two-CTA N = 2048 instance
+// (pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1>, lane-pair layout: same phase
+// functions, same order, same barriers) with a clock64() read between phases,
+// for exchange 2 through the warp's own rows (x2m_*, X2 = 1, the shipped one)
+// and through half-warp shuffles (x2h_*, X2 = 0).  Every SM runs 1 or 2 CTAs;
+// the tool prints the average cycles per phase of warp 0 of CTA 0.  The clock
+// reads order the phases of a warp, so the sum is a little above the step time
+// of the kernel.  Measurement tool only (not part of the library).
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I../../tfhe-rs_b200/csrc -o phase_clocks phase_clocks.cu
+//   ./phase_clocks <CTAs per SM: 1 or 2>
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -17,128 +22,109 @@ __device__ __forceinline__ long long clk() {
   return c;
 }
 
+template <int X2>
 __global__ void __launch_bounds__(128, 2)
-timed_kernel(const cplx *__restrict__ bsk, const Fft1024Tables *__restrict__ tables,
-             uint32_t n, uint32_t base_log, unsigned long long *out) {
+timed_lanepair(const cplx *__restrict__ bsk, const Fft1024Tables *__restrict__ tables,
+               uint32_t n, uint32_t base_log, unsigned long long *out) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  P22SmemV3 &sm = *reinterpret_cast<P22SmemV3 *>(smem_raw);
-  const int tid = threadIdx.x, g = tid >> 6, t = tid & 63;
-  for (uint32_t i = tid; i < n; i += 128)
+  using Smem = P22SmemV6<2, true>;
+  Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
+  const int tid = threadIdx.x;
+  const int g = (tid >> 4) & 1, t = ((tid >> 5) << 4) | (tid & 15);
+  if (tid == 0) { mbar_init(&sm.bar, 1); mbar_fence_init(); }
+  for (uint32_t i = tid; i < n + 8; i += 128)
     sm.a_hat[i] = (uint16_t)(1 + ((i * 2654435761u + blockIdx.x * 40503u) % 4095u));
   for (uint32_t j = tid; j < 2 * P22_N; j += 128)
     sm.acc[j >> 11][j & (P22_N - 1)] = j * 2654435761u + blockIdx.x;
   cplx tw2[3], tw3[15];
 #pragma unroll
-  for (int e = 0; e < 3; e++) tw2[e] = tables->pass2[t >> 2][e];
+  for (int e = 0; e < 3; e++) tw2[e] = tables->pass2[x1h_q(t)][e];
 #pragma unroll
   for (int e = 0; e < 15; e++) tw3[e] = tables->pass3[t][e];
   __syncthreads();
+  auto tma_issue = [&](uint32_t i) {
+    mbar_arrive_expect_tx(&sm.bar, 2u * P22_M * (uint32_t)sizeof(cplx));
+    tma_bulk_g2s(&sm.ring[0][0], bsk + (size_t)i * (4 * P22_M) + P22_M,
+                 2u * P22_M * (uint32_t)sizeof(cplx), &sm.bar);
+  };
+  if (tid == 0) tma_issue(0);
+  __syncthreads();
   uint32_t *acc_g = sm.acc[g];
-  cplx *xa_g = sm.xa[g], *xb_g = sm.xb[g];
-  const cplx *xa_other = sm.xa[1 - g];
+  cplx *xa_g = sm.xa[g];
+  cplx *x2_rows = xa_g + 256 * (tid >> 5);
+  const cplx *k_oth = &sm.ring[g][0];
   const cplx *bsk_own = bsk + (size_t)g * (2 * P22_M) + (size_t)g * P22_M + t;
-  const cplx *bsk_oth = bsk + (size_t)g * (2 * P22_M) + (size_t)(1 - g) * P22_M;
-  long long acc[NPH];
+  uint32_t own[32];
+  p22v4_own_init(acc_g, t, own);
+  uint32_t acc[NPH]; // 32-bit sums (918 steps of a few thousand cycles) keep the replay free of spills
   for (int p = 0; p < NPH; p++) acc[p] = 0;
   long long t0, t1;
-#define LAP(p) t1 = clk(); acc[p] += t1 - t0; t0 = t1;
+#define LAP(p) t1 = clk(); acc[p] += (uint32_t)(t1 - t0); t0 = t1;
+  uint32_t a_next = sm.a_hat[0];
   for (uint32_t i = 0; i < n; i++) {
-    const uint32_t a = sm.a_hat[i];
-    const size_t step = (size_t)i * (4 * P22_M);
-    cplx v[16], b_own[16];
+    const uint32_t a = a_next;
+    a_next = sm.a_hat[i + 1];
+    cplx v[16];
     t0 = clk();
-    p22v3_load_digits(acc_g, t, a, base_log, v);        LAP(0)
-    radix16_fwd(v, c_fft1024_pass1);                    LAP(1)
-    x1_store_p1(xa_g, t, v); group_barrier(g); x1_load_p2(xa_g, t, v); LAP(2)
-    pass2_fwd(v, tw2);                                  LAP(3)
-    x2_store_p2(xb_g, t, v); group_barrier(g); x2_load_p3(xb_g, t, v); LAP(4)
-    radix16_fwd(v, tw3);                                LAP(5)
+    p22v4_load_digits<2>(acc_g, t, a, base_log, own, v);        LAP(0)
+    radix16_fwd(v, c_fft1024_pass1);                            LAP(1)
+    x1h_store_p1(xa_g, t, v); __syncthreads(); x1h_load_p2(xa_g, t, v); LAP(2)
+    pass2_fwd(v, tw2);                                          LAP(3)
+    if constexpr (X2 == 1) x2m_fwd(x2_rows, v); else x2h_fwd(v); LAP(4)
+    radix16_fwd(v, tw3);                                        LAP(5)
+    const size_t step = (size_t)i * (4 * P22_M);
+    cplx b_own[16];
 #pragma unroll
     for (int b = 0; b < 16; b++) b_own[b] = ldcg_cplx(bsk_own + step + b * 64);
-    spec_store(xa_g, t, v); __syncthreads();            LAP(6)
-    p22v3_mac(v, b_own, xa_other, bsk_oth + step, t, LdcgLoader()); LAP(7)
-    __syncthreads();                                    LAP(8)
-    radix16_inv(v, tw3);                                LAP(9)
-    x2_store_p3(xb_g, t, v); group_barrier(g); x2_load_p2(xb_g, t, v); LAP(10)
-    pass2_inv(v, tw2);                                  LAP(11)
-    x1_store_p2(xa_g, t, v); group_barrier(g); x1_load_p1(xa_g, t, v); LAP(12)
-    radix16_inv(v, c_fft1024_pass1);                    LAP(13)
-    p22v2_acc_update(acc_g, t, v); group_barrier(g);    LAP(14)
+    mbar_wait_parity(&sm.bar, i & 1u);                          LAP(6)
+#pragma unroll
+    for (int b = 0; b < 16; b++) {
+      const cplx o = shfl_xor_cplx(v[b], 16);
+      v[b] = cfma(o, k_oth[b * 64 + t], cmul(v[b], b_own[b]));
+    }
+    LAP(7)
+    radix16_inv(v, tw3);                                        LAP(8)
+    if constexpr (X2 == 1) x2m_inv(x2_rows, v); else x2h_inv(v); LAP(9)
+    pass2_inv(v, tw2);                                          LAP(10)
+    __syncwarp(); x1h_store_p2(xa_g, t, v); __syncthreads();
+    if (tid == 0 && i + 1 < n) tma_issue(i + 1);
+    x1h_load_p1(xa_g, t, v);                                    LAP(11)
+    radix16_inv(v, c_fft1024_pass1);                            LAP(12)
+    p22v4_acc_update(acc_g, t, v, own); __syncthreads();        LAP(13)
   }
   if (tid == 0 && blockIdx.x == 0)
     for (int p = 0; p < NPH; p++) out[p] = (unsigned long long)acc[p];
   if (sm.acc[0][tid] == 0x12345678u) out[NPH] = 1; // keep results live
 }
 
-// the same replay for the v6 kernel: exchange 2 through warp shuffles, key
-// block of the step from the one-slot TMA ring (pbs_n2048_k1_l1_v6_kernel<0>)
-__global__ void __launch_bounds__(128, 2)
-timed_kernel_v6(const cplx *__restrict__ bsk, const Fft1024Tables *__restrict__ tables,
-                uint32_t n, uint32_t base_log, unsigned long long *out) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  P22SmemV6<4, false> &sm = *reinterpret_cast<P22SmemV6<4, false> *>(smem_raw);
-  const int tid = threadIdx.x, g = tid >> 6, t = tid & 63;
-  if (tid == 0) { mbar_init(&sm.bar, 1); mbar_fence_init(); }
-  for (uint32_t j = tid; j < 2 * P22_N; j += 128)
-    sm.acc[j >> 11][j & (P22_N - 1)] = j * 2654435761u + blockIdx.x;
-  cplx tw2[3], tw3[15];
-#pragma unroll
-  for (int e = 0; e < 3; e++) tw2[e] = tables->pass2[x1t_q(t)][e];
-#pragma unroll
-  for (int e = 0; e < 15; e++) tw3[e] = tables->pass3[t][e];
-  __syncthreads();
-  auto tma_issue = [&](uint32_t i) {
-    mbar_arrive_expect_tx(&sm.bar, 4u * P22_M * (uint32_t)sizeof(cplx));
-#pragma unroll
-    for (int q = 0; q < 4; q++)
-      tma_bulk_g2s(&sm.ring[q][0], bsk + (size_t)i * (4 * P22_M) + (size_t)q * P22_M,
-                   P22_M * (uint32_t)sizeof(cplx), &sm.bar);
-  };
-  if (tid == 0) tma_issue(0);
-  uint32_t *acc_g = sm.acc[g];
-  cplx *xa_g = sm.xa[g];
-  const cplx *xa_other = sm.xa[1 - g];
-  const cplx *k_own = &sm.ring[2 * g + g][0];
-  const cplx *k_oth = &sm.ring[2 * g + (1 - g)][0];
-  uint32_t own[32];
-  p22v4_own_init(acc_g, t, own);
-  long long acc[NPH];
-  for (int p = 0; p < NPH; p++) acc[p] = 0;
-  long long t0, t1;
-  for (uint32_t i = 0; i < n; i++) {
-    const uint32_t a = 1 + ((i * 2654435761u + blockIdx.x * 40503u) % 4095u);
-    cplx v[16];
-    t0 = clk();
-    p22v4_load_digits(acc_g, t, a, base_log, own, v);   LAP(0)
-    radix16_fwd(v, c_fft1024_pass1);                    LAP(1)
-    x1t_store_p1(xa_g, t, v); group_barrier(g); x1t_load_p2(xa_g, t, v); LAP(2)
-    pass2_fwd(v, tw2); spec_guard_arrive(g, t);         LAP(3)
-    x2s_fwd(v);                                         LAP(4)
-    radix16_fwd(v, tw3);                                LAP(5)
-    spec_guard_wait(g, t); spec_store(xa_g, t, v); __syncthreads(); LAP(6)
-    mbar_wait_parity(&sm.bar, i & 1u);
-#pragma unroll
-    for (int b = 0; b < 16; b++)
-      v[b] = cfma(xa_other[b * 64 + t], k_oth[b * 64 + t], cmul(v[b], k_own[b * 64 + t]));
-    LAP(7)
-    __syncthreads();
-    if (tid == 0 && i + 1 < n) tma_issue(i + 1);
-    LAP(8)
-    radix16_inv(v, tw3);                                LAP(9)
-    x2s_inv(v);                                         LAP(10)
-    pass2_inv(v, tw2);                                  LAP(11)
-    x1t_store_p2(xa_g, t, v); group_barrier(g); x1t_load_p1(xa_g, t, v); LAP(12)
-    radix16_inv(v, c_fft1024_pass1);                    LAP(13)
-    p22v4_acc_update(acc_g, t, v, own); group_barrier(g); LAP(14)
+template <int X2>
+static int run(const char *label, int ctas, int sms, const cplx *bsk, const Fft1024Tables *dt, uint32_t n,
+               unsigned long long *out) {
+  const int smem = (int)sizeof(P22SmemV6<2, true>);
+  cudaFuncSetAttribute(timed_lanepair<X2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  for (int rep = 0; rep < 2; rep++) {
+    timed_lanepair<X2><<<ctas * sms, 128, smem>>>(bsk, dt, n, 23, out);
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) { printf("error %s\n", cudaGetErrorString(e)); return 1; }
   }
-  if (tid == 0 && blockIdx.x == 0)
-    for (int p = 0; p < NPH; p++) out[p] = (unsigned long long)acc[p];
-  if (sm.acc[0][tid] == 0x12345678u) out[NPH] = 1;
+  unsigned long long h[NPH + 1];
+  cudaMemcpy(h, out, sizeof(h), cudaMemcpyDeviceToHost);
+  const char *names[14] = {"digits (rotate + decompose)", "fwd pass 1", "exchange 1 (+ CTA barrier)", "fwd pass 2",
+                           "exchange 2", "fwd pass 3", "own-row key load + key wait", "MAC", "inv pass 3",
+                           "inv exchange 2", "inv pass 2", "inv exchange 1 (+ CTA barrier, TMA issue)", "inv pass 1",
+                           "accumulator update (+ CTA barrier)"};
+  unsigned long long tot = 0;
+  for (int p = 0; p < 14; p++) tot += h[p];
+  printf("%s, %d CTA(s) per SM: %.0f cycles per CMUX step (warp 0 of CTA 0)\n", label, ctas, (double)tot / n);
+  for (int p = 0; p < 14; p++) printf("  %-44s %7.0f  %5.1f %%\n", names[p], (double)h[p] / n, 100.0 * h[p] / tot);
+  return 0;
 }
 
 int main(int argc, char **argv) {
   const uint32_t n = 918;
-  const int ctas = argc > 1 ? atoi(argv[1]) : 1;
+  const int ctas = argc > 1 ? atoi(argv[1]) : 2;
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   Fft1024Tables *host = new Fft1024Tables;
   b200_fill_fft1024_tables(host);
   Fft1024Tables *dt;
@@ -147,27 +133,11 @@ int main(int argc, char **argv) {
   cudaMemcpyToSymbol(c_fft1024_pass1, host->pass1, sizeof(host->pass1));
   const size_t words = (size_t)n * 4 * P22_M;
   std::vector<cplx> h(words);
-  for (size_t i = 0; i < words; i++) { h[i].re = 1e-9 * (double)((i * 2654435761u) % 1000) ; h[i].im = -h[i].re; }
+  for (size_t i = 0; i < words; i++) { h[i].re = 1e-9 * (double)((i * 2654435761u) % 1000); h[i].im = -h[i].re; }
   cplx *bsk; cudaMalloc(&bsk, words * sizeof(cplx));
   cudaMemcpy(bsk, h.data(), words * sizeof(cplx), cudaMemcpyHostToDevice);
   unsigned long long *out; cudaMalloc(&out, (NPH + 1) * 8); cudaMemset(out, 0, (NPH + 1) * 8);
-  const bool v6 = argc > 2 && atoi(argv[2]) == 6;
-  cudaFuncSetAttribute(timed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(P22SmemV3));
-  cudaFuncSetAttribute(timed_kernel_v6, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(P22SmemV6<4, false>));
-  for (int rep = 0; rep < 2; rep++) {
-    if (v6) timed_kernel_v6<<<ctas, 128, sizeof(P22SmemV6<4, false>)>>>(bsk, dt, n, 23, out);
-    else timed_kernel<<<ctas, 128, sizeof(P22SmemV3)>>>(bsk, dt, n, 23, out);
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { printf("error %s\n", cudaGetErrorString(e)); return 1; }
-  }
-  unsigned long long hout[NPH + 1];
-  cudaMemcpy(hout, out, sizeof(hout), cudaMemcpyDeviceToHost);
-  const char *names[NPH] = {"load_digits", "fwd pass1 (radix16)", "exchange 1", "fwd pass2 (radix4)", "exchange 2",
-    "fwd pass3 (radix16)", "key prefetch issue + spectrum share + syncthreads", "MAC", "syncthreads", "inv pass3",
-    "exchange 2'", "inv pass2", "exchange 1'", "inv pass1", "acc update + barrier", ""};
-  unsigned long long tot = 0;
-  for (int p = 0; p < 15; p++) tot += hout[p];
-  printf("%s, CTAs %d: %.0f cycles per CMUX step (warp 0 of CTA 0)\n", v6 ? "v6 (shuffle exchange 2, TMA key ring)" : "v3", ctas, (double)tot / n);
-  for (int p = 0; p < 15; p++) printf("  %-52s %7.0f  %5.1f %%\n", names[p], (double)hout[p] / n, 100.0 * hout[p] / tot);
+  if (run<0>("lane-pair, exchange 2 through half-warp shuffles (x2h)", ctas, sms, bsk, dt, n, out)) return 1;
+  if (run<1>("lane-pair, exchange 2 through the warp's rows (x2m)", ctas, sms, bsk, dt, n, out)) return 1;
   return 0;
 }
