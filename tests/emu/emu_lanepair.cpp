@@ -69,26 +69,13 @@ void emu_pbs_p22_lanepair(const double *bsk_, const uint64_t *lut, const uint64_
   std::vector<uint32_t> acc(2 * ACC_STRIDE);
   std::vector<cplx> xa(2 * P22_M);
   std::vector<uint16_t> a_hat(n);
-  uint64_t half_sum = 0;
-  int64_t dbl_sum = 0;
+  CenteredMsSums sums;
   for (uint32_t i = 0; i < n; i++) {
     a_hat[i] = (uint16_t)modulus_switch_u64(ct[i], log_mod);
-    if (centered_ms) {
-      int64_t d;
-      half_sum += (uint64_t)centered_ms_half_error(ct[i], log_mod, &d);
-      dbl_sum += d;
-    }
+    sums.add(ct[i], log_mod);
   }
-  uint64_t body = ct[n];
-  if (centered_ms) {
-    half_sum -= (uint64_t)(dbl_sum / 2);
-    body += half_sum - ((uint64_t)1 << (63 - log_mod));
-  }
-  const uint32_t b_hat = modulus_switch_u64(body, log_mod);
-  for (uint32_t j = 0; j < 2 * P22_N; j++) {
-    const uint32_t r = j >> 11, jj = j & (P22_N - 1);
-    acc[r * ACC_STRIDE + jj] = torus64_to_32(rot_div_coeff(lut + r * P22_N, P22_N, jj, b_hat));
-  }
+  const uint32_t b_hat = ms_b_hat(ct[n], centered_ms, &sums.half, &sums.dbl, 1, log_mod);
+  rotate_lut(acc.data(), ACC_STRIDE, lut, 2, P22_N, b_hat, 0, 1, Torus64To32());
   std::vector<Lane> R(128);
   auto acc_of = [&](int tid) { return acc.data() + lane_g(tid) * ACC_STRIDE; };
   auto xa_of = [&](int tid) { return xa.data() + lane_g(tid) * P22_M; };
@@ -137,16 +124,8 @@ void emu_pbs_p22_lanepair(const double *bsk_, const uint64_t *lut, const uint64_
       p22v4_acc_update(acc_of(tid), lane_t(tid), R[tid].v, R[tid].own);
     }
   }
-  const uint64_t out_len = P22_N + 1;
-  for (uint32_t m = 0; m < num_many_lut; m++) {
-    const uint32_t nth = m * lut_stride;
-    uint64_t *out = out_base + (uint64_t)m * count * out_len;
-    for (uint32_t tt = 0; tt < P22_N; tt++) {
-      const uint32_t x = tt <= nth ? acc[nth - tt] : 0u - acc[P22_N + nth - tt];
-      out[tt] = (uint64_t)x << 32;
-    }
-    out[P22_N] = (uint64_t)acc[ACC_STRIDE + nth] << 32;
-  }
+  sample_extract_many_lut(out_base, 0, count, num_many_lut, lut_stride, acc.data(),
+                          ACC_STRIDE, 1, P22_N, 0, 1, Torus32To64());
 }
 
 // Bank-conflict audit of the lane-pair layout.

@@ -301,26 +301,13 @@ void emu_pbs_p22(const double *bsk_, const uint64_t *lut, const uint64_t *ct,
   std::vector<cplx> xa(2 * P22_M), xb(2 * P22_M);
   std::vector<uint16_t> a_hat(n);
   // prologue
-  uint64_t half_sum = 0;
-  int64_t dbl_sum = 0;
+  CenteredMsSums sums;
   for (uint32_t i = 0; i < n; i++) {
     a_hat[i] = (uint16_t)modulus_switch_u64(ct[i], log_mod);
-    if (centered_ms) {
-      int64_t d;
-      half_sum += (uint64_t)centered_ms_half_error(ct[i], log_mod, &d);
-      dbl_sum += d;
-    }
+    sums.add(ct[i], log_mod);
   }
-  uint64_t body = ct[n];
-  if (centered_ms) {
-    half_sum -= (uint64_t)(dbl_sum / 2);
-    body += half_sum - ((uint64_t)1 << (63 - log_mod));
-  }
-  const uint32_t b_hat = modulus_switch_u64(body, log_mod);
-  for (uint32_t j = 0; j < 2 * P22_N; j++) {
-    const uint32_t r = j >> 11, jj = j & (P22_N - 1);
-    acc[j] = rot_div_coeff(lut + r * P22_N, P22_N, jj, b_hat);
-  }
+  const uint32_t b_hat = ms_b_hat(ct[n], centered_ms, &sums.half, &sums.dbl, 1, log_mod);
+  rotate_lut(acc.data(), P22_N, lut, 2, P22_N, b_hat, 0, 1, SameWord());
   std::vector<Regs> R(128);
   std::vector<cplx> tw2(128 * 12), tw3(128 * 15);
   for (int tid = 0; tid < 128; tid++) {
@@ -378,14 +365,8 @@ void emu_pbs_p22(const double *bsk_, const uint64_t *lut, const uint64_t *ct,
       p22_acc_update(acc_g, t, v);
     END_THREADS
   }
-  const uint64_t out_len = P22_N + 1;
-  for (uint32_t m = 0; m < num_many_lut; m++) {
-    const uint32_t nth = m * lut_stride;
-    uint64_t *out = out_base + (uint64_t)m * count * out_len;
-    for (uint32_t tt = 0; tt < P22_N; tt++)
-      out[tt] = sample_extract_mask_coeff(acc.data(), P22_N, nth, tt);
-    out[P22_N] = acc[P22_N + nth];
-  }
+  sample_extract_many_lut(out_base, 0, count, num_many_lut, lut_stride, acc.data(), P22_N,
+                          1, P22_N, 0, 1, SameWord());
 }
 
 // mirrors pbs_n2048_k1_l1_v3_kernel (u32 accumulator, lean digits, prefetch MAC)
@@ -399,26 +380,13 @@ void emu_pbs_p22_v3(const double *bsk_, const uint64_t *lut, const uint64_t *ct,
   std::vector<uint32_t> acc(2 * P22_N);
   std::vector<cplx> xa(2 * P22_M);
   std::vector<uint16_t> a_hat(n);
-  uint64_t half_sum = 0;
-  int64_t dbl_sum = 0;
+  CenteredMsSums sums;
   for (uint32_t i = 0; i < n; i++) {
     a_hat[i] = (uint16_t)modulus_switch_u64(ct[i], log_mod);
-    if (centered_ms) {
-      int64_t d;
-      half_sum += (uint64_t)centered_ms_half_error(ct[i], log_mod, &d);
-      dbl_sum += d;
-    }
+    sums.add(ct[i], log_mod);
   }
-  uint64_t body = ct[n];
-  if (centered_ms) {
-    half_sum -= (uint64_t)(dbl_sum / 2);
-    body += half_sum - ((uint64_t)1 << (63 - log_mod));
-  }
-  const uint32_t b_hat = modulus_switch_u64(body, log_mod);
-  for (uint32_t j = 0; j < 2 * P22_N; j++) {
-    const uint32_t r = j >> 11, jj = j & (P22_N - 1);
-    acc[j] = torus64_to_32(rot_div_coeff(lut + r * P22_N, P22_N, jj, b_hat));
-  }
+  const uint32_t b_hat = ms_b_hat(ct[n], centered_ms, &sums.half, &sums.dbl, 1, log_mod);
+  rotate_lut(acc.data(), P22_N, lut, 2, P22_N, b_hat, 0, 1, Torus64To32());
   std::vector<Regs> R(128);
 #define FOR_THREADS2                                                           \
   for (int tid = 0; tid < 128; tid++) {                                        \
@@ -486,16 +454,8 @@ void emu_pbs_p22_v3(const double *bsk_, const uint64_t *lut, const uint64_t *ct,
       p22v4_acc_update(acc_g, t, v, R[tid].own);
     END_THREADS
   }
-  const uint64_t out_len = P22_N + 1;
-  for (uint32_t m = 0; m < num_many_lut; m++) {
-    const uint32_t nth = m * lut_stride;
-    uint64_t *out = out_base + (uint64_t)m * count * out_len;
-    for (uint32_t tt = 0; tt < P22_N; tt++) {
-      const uint32_t x = tt <= nth ? acc[nth - tt] : 0u - acc[P22_N + nth - tt];
-      out[tt] = (uint64_t)x << 32;
-    }
-    out[P22_N] = (uint64_t)acc[P22_N + nth] << 32;
-  }
+  sample_extract_many_lut(out_base, 0, count, num_many_lut, lut_stride, acc.data(), P22_N,
+                          1, P22_N, 0, 1, Torus32To64());
 }
 
 // bank-conflict audit of the exchange layouts: for each of the 8 access
@@ -669,16 +629,8 @@ static void emu_pbs_mb_impl(const cplx *bsk, const uint64_t *lut,
       acc[g * P22_N + 64 * j1 + t + P22_M] = R[tid].hi[j1];
     }
   }
-  const uint64_t out_len = P22_N + 1;
-  for (uint32_t m = 0; m < num_many_lut; m++) {
-    const uint32_t nth = m * lut_stride;
-    uint64_t *out = out_base + (uint64_t)m * count * out_len;
-    for (uint32_t tt = 0; tt < P22_N; tt++) {
-      const uint32_t x = tt <= nth ? acc[nth - tt] : 0u - acc[P22_N + nth - tt];
-      out[tt] = (uint64_t)x << 32;
-    }
-    out[P22_N] = (uint64_t)acc[P22_N + nth] << 32;
-  }
+  sample_extract_many_lut(out_base, 0, count, num_many_lut, lut_stride, acc.data(), P22_N,
+                          1, P22_N, 0, 1, Torus32To64());
 }
 
 extern "C" void emu_pbs_mb(const double *bsk_, const uint64_t *lut, const uint64_t *ct,
@@ -729,27 +681,13 @@ extern "C" void emu_pbs_n8192(const double *bsk_, const uint64_t *lut, const uin
   std::vector<std::vector<cplx>> spec(4, std::vector<cplx>(P8K_M));
   for (uint32_t s = 0; s < count; s++) {
     const uint64_t *ct = cts + (size_t)s * (n + 1);
-    unsigned long long half_sum = 0;
-    long long dbl_sum = 0;
+    CenteredMsSums sums;
     for (uint32_t i = 0; i < n; i++) {
       a_hat[i] = modulus_switch_u64(ct[i], log_mod) & 0xFFFFu;
-      if (centered_ms) {
-        int64_t dd;
-        half_sum += (unsigned long long)centered_ms_half_error(ct[i], log_mod, &dd);
-        dbl_sum += dd;
-      }
+      sums.add(ct[i], log_mod);
     }
-    uint64_t body = ct[n];
-    if (centered_ms) {
-      uint64_t hs = half_sum;
-      hs -= (uint64_t)(dbl_sum / 2);
-      body += hs - ((uint64_t)1 << (63 - log_mod));
-    }
-    const uint32_t b_hat = modulus_switch_u64(body, log_mod);
-    for (uint32_t j = 0; j < 2 * P8K_N; j++) {
-      const uint32_t r = j >> 13, jj = j & (P8K_N - 1);
-      acc[j] = torus64_to_32(rot_div_coeff(lut + r * P8K_N, P8K_N, jj, b_hat));
-    }
+    const uint32_t b_hat = ms_b_hat(ct[n], centered_ms, &sums.half, &sums.dbl, 1, log_mod);
+    rotate_lut(acc.data(), P8K_N, lut, 2, P8K_N, b_hat, 0, 1, Torus64To32());
     for (uint32_t i = 0; i < n; i++) {
       const uint32_t a = a_hat[i];
       if (a == 0)
@@ -785,15 +723,8 @@ extern "C" void emu_pbs_n8192(const double *bsk_, const uint64_t *lut, const uin
         }
       }
     }
-    for (uint32_t m = 0; m < num_many_lut; m++) {
-      const uint32_t nth = m * lut_stride;
-      uint64_t *o = out_base + ((size_t)m * count + s) * (P8K_N + 1);
-      for (uint32_t tt = 0; tt < P8K_N; tt++) {
-        const uint32_t x = tt <= nth ? acc[nth - tt] : 0u - acc[P8K_N + nth - tt];
-        o[tt] = (uint64_t)x << 32;
-      }
-      o[P8K_N] = (uint64_t)acc[P8K_N + nth] << 32;
-    }
+    sample_extract_many_lut(out_base, s, count, num_many_lut, lut_stride, acc.data(), P8K_N,
+                            1, P8K_N, 0, 1, Torus32To64());
   }
 }
 

@@ -26,17 +26,7 @@ glwe_sample_extract_kernel(uint64_t *__restrict__ lwe_out,
   const uint64_t *glwe = glwe_in + (uint64_t)(id / per_glwe) * (k + 1) * N;
   uint64_t *out = lwe_out + (uint64_t)id * ((uint64_t)k * N + 1);
   const uint32_t nth = nth_array[id] % stored_per_glwe;
-  for (uint32_t w = threadIdx.x; w < k * N; w += blockDim.x) {
-    const uint32_t p = w / N, t = w % N;
-    out[w] = sample_extract_mask_coeff(glwe + (uint64_t)p * N, N, nth, t);
-  }
-  if (threadIdx.x == 0)
-    out[(uint64_t)k * N] = glwe[(uint64_t)k * N + nth];
-}
-
-__device__ __forceinline__ uint64_t modulus_switch_full(uint64_t x,
-                                                        uint32_t log_modulus) {
-  return (x + ((uint64_t)1 << (63 - log_modulus))) >> (64 - log_modulus);
+  sample_extract_lwe(out, glwe, N, k, N, nth, threadIdx.x, blockDim.x, SameWord());
 }
 
 __global__ void __launch_bounds__(256)
@@ -55,36 +45,17 @@ centered_modulus_switch_kernel(uint64_t *__restrict__ out,
                                uint32_t log_modulus) {
   __shared__ unsigned long long red_half[8];
   __shared__ long long red_dbl[8];
-  unsigned long long half_sum = 0;
-  long long dbl_sum = 0;
+  CenteredMsSums sums;
   for (uint32_t i = threadIdx.x; i < n; i += 256) {
     const uint64_t a = in[i];
     out[i] = modulus_switch_full(a, log_modulus);
-    int64_t d;
-    half_sum += (unsigned long long)centered_ms_half_error(a, log_modulus, &d);
-    dbl_sum += d;
+    sums.add(a, log_modulus);
   }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) {
-    half_sum += __shfl_xor_sync(0xffffffffu, half_sum, off);
-    dbl_sum += __shfl_xor_sync(0xffffffffu, dbl_sum, off);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    red_half[threadIdx.x >> 5] = half_sum;
-    red_dbl[threadIdx.x >> 5] = dbl_sum;
-  }
+  centered_ms_publish_warp(sums, red_half, red_dbl);
   __syncthreads();
-  if (threadIdx.x == 0) {
-    uint64_t hs = 0;
-    int64_t ds = 0;
-    for (int w = 0; w < 8; w++) {
-      hs += red_half[w];
-      ds += red_dbl[w];
-    }
-    hs -= (uint64_t)(ds / 2);
-    const uint64_t body = in[n] + hs - ((uint64_t)1 << (63 - log_modulus));
-    out[n] = modulus_switch_full(body, log_modulus);
-  }
+  if (threadIdx.x == 0)
+    out[n] = modulus_switch_full(centered_ms_body(in[n], red_half, red_dbl, 8, log_modulus),
+                                 log_modulus);
 }
 
 } // namespace b200

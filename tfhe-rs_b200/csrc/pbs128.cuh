@@ -63,54 +63,21 @@ pbs128_kernel(u128 *__restrict__ lwe_out, const u128 *__restrict__ lut,
   for (uint32_t s = blockIdx.x; s < num_samples; s += gridDim.x) {
     const uint64_t *ct = lwe_in + (uint64_t)s * (n + 1);
     // ---- modulus switch (same as the 64-bit PBS) ---------------------------
-    unsigned long long half_sum = 0;
-    long long dbl_sum = 0;
+    CenteredMsSums sums;
     for (uint32_t i = tid; i < n; i += NT) {
       const uint64_t a = ct[i];
       a_hat[i] = modulus_switch_u64(a, log_mod);
-      if (centered_ms) {
-        int64_t d;
-        half_sum += (unsigned long long)centered_ms_half_error(a, log_mod, &d);
-        dbl_sum += d;
-      }
+      if (centered_ms)
+        sums.add(a, log_mod);
     }
-    if (centered_ms) {
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) {
-        half_sum += __shfl_xor_sync(0xffffffffu, half_sum, off);
-        dbl_sum += __shfl_xor_sync(0xffffffffu, dbl_sum, off);
-      }
-      if ((tid & 31) == 0) {
-        red_half[tid >> 5] = half_sum;
-        red_dbl[tid >> 5] = dbl_sum;
-      }
-    }
+    if (centered_ms)
+      centered_ms_publish_warp(sums, red_half, red_dbl);
     __syncthreads();
-    if (tid == 0) {
-      uint64_t body = ct[n];
-      if (centered_ms) {
-        uint64_t hs = 0;
-        int64_t ds = 0;
-        for (uint32_t w = 0; w < NT / 32; w++) {
-          hs += red_half[w];
-          ds += red_dbl[w];
-        }
-        hs -= (uint64_t)(ds / 2);
-        body += hs - ((uint64_t)1 << (63 - log_mod));
-      }
-      b_hat_s = modulus_switch_u64(body, log_mod);
-    }
+    if (tid == 0)
+      b_hat_s = ms_b_hat(ct[n], centered_ms, red_half, red_dbl, NT / 32, log_mod);
     __syncthreads();
     // ---- acc = LUT * X^{-b_hat} ------------------------------------------------
-    {
-      const uint32_t b_hat = b_hat_s, d = b_hat & (N - 1);
-      for (uint32_t j = tid; j < (k + 1) * N; j += NT) {
-        const uint32_t r = j / N, jj = j % N, sj = jj + d;
-        const bool wrap = sj >= N;
-        const u128 x = lut[(size_t)r * N + (wrap ? sj - N : sj)];
-        acc[j] = ((b_hat >= N) != wrap) ? (u128)0 - x : x;
-      }
-    }
+    rotate_lut(acc, N, lut, k + 1, N, b_hat_s, tid, NT, SameWord());
     __syncthreads();
 
     // ---- blind rotation ----------------------------------------------------------
@@ -148,14 +115,8 @@ pbs128_kernel(u128 *__restrict__ lwe_out, const u128 *__restrict__ lut,
     }
 
     // ---- sample extraction of coefficient 0 --------------------------------------
-    u128 *o = lwe_out + (uint64_t)s * ((uint64_t)k * N + 1);
-    for (uint32_t w = tid; w < k * N; w += NT) {
-      const uint32_t r = w / N, tt = w % N;
-      const u128 *A = acc + (size_t)r * N;
-      o[w] = tt == 0 ? A[0] : (u128)0 - A[N - tt];
-    }
-    if (tid == 0)
-      o[(size_t)k * N] = acc[(size_t)k * N];
+    sample_extract_lwe(lwe_out + (uint64_t)s * ((uint64_t)k * N + 1), acc, N, k, N, 0,
+                       tid, NT, SameWord());
     __syncthreads(); // the workspace is reused by the next sample of this CTA
   }
 }

@@ -99,58 +99,24 @@ pbs_generic_kernel(Torus *__restrict__ lwe_out,
   const Torus *ct = lwe_in + (uint64_t)in_idx[s] * (uint64_t)(n + 1);
 
   // ---- modulus switch --------------------------------------------------
-  unsigned long long half_sum = 0;
-  long long dbl_sum = 0;
   if (!multibit) {
+    CenteredMsSums sums;
     for (uint32_t i = tid; i < n; i += NTHREADS) {
       const uint64_t a = Io::widen(ct[i]);
       a_hat[i] = modulus_switch_u64(a, log_mod);
-      if (centered_ms) {
-        int64_t d;
-        half_sum += (unsigned long long)centered_ms_half_error(a, log_mod, &d);
-        dbl_sum += d;
-      }
+      if (centered_ms)
+        sums.add(a, log_mod);
     }
-    if (centered_ms) {
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) {
-        half_sum += __shfl_xor_sync(0xffffffffu, half_sum, off);
-        dbl_sum += __shfl_xor_sync(0xffffffffu, dbl_sum, off);
-      }
-      if ((tid & 31) == 0) {
-        red_half[tid >> 5] = half_sum;
-        red_dbl[tid >> 5] = dbl_sum;
-      }
-    }
+    if (centered_ms)
+      centered_ms_publish_warp(sums, red_half, red_dbl);
   }
   __syncthreads();
-  if (tid == 0) {
-    uint64_t body = Io::widen(ct[n]);
-    if (!multibit && centered_ms) {
-      uint64_t hs = 0;
-      int64_t ds = 0;
-      for (int w = 0; w < NTHREADS / 32; w++) {
-        hs += red_half[w];
-        ds += red_dbl[w];
-      }
-      hs -= (uint64_t)(ds / 2);
-      body += hs - ((uint64_t)1 << (63 - log_mod));
-    }
-    b_hat_s = modulus_switch_u64(body, log_mod);
-  }
+  if (tid == 0)
+    b_hat_s = ms_b_hat(Io::widen(ct[n]), !multibit && centered_ms, red_half, red_dbl,
+                       NTHREADS / 32, log_mod);
   __syncthreads();
-  {
-    const Torus *lut = luts + (uint64_t)lut_idx[s] * (uint64_t)((k + 1) * N);
-    const uint32_t b_hat = b_hat_s;
-    for (uint32_t j = tid; j < (k + 1) * N; j += NTHREADS) {
-      const uint32_t r = j / N, jj = j % N;
-      // LUT * X^{-b_hat} (polynomial_wrapping_monic_monomial_div)
-      const uint32_t d = b_hat & (N - 1), sj = jj + d;
-      const bool wrap = sj >= N;
-      const uint64_t x = Io::widen(lut[(size_t)r * N + (wrap ? sj - N : sj)]);
-      acc[j] = ((b_hat >= N) != wrap) ? (uint64_t)0 - x : x;
-    }
-  }
+  rotate_lut(acc, N, luts + (uint64_t)lut_idx[s] * (uint64_t)((k + 1) * N), k + 1, N,
+             b_hat_s, tid, NTHREADS, [](Torus x) { return Io::widen(x); });
   __syncthreads();
 
   const uint32_t nggsw = multibit ? (1u << grouping) : 1u;
@@ -192,19 +158,9 @@ pbs_generic_kernel(Torus *__restrict__ lwe_out,
     __syncthreads();
   }
 
-  const uint64_t out_len = (uint64_t)k * N + 1;
-  for (uint32_t m = 0; m < num_many_lut; m++) {
-    const uint32_t nth = m * lut_stride;
-    Torus *o =
-        lwe_out + ((uint64_t)m * num_samples + (uint64_t)out_idx[s]) * out_len;
-    for (uint32_t w = tid; w < k * N; w += NTHREADS) {
-      const uint32_t r = w / N, tt = w % N;
-      o[w] = Io::narrow(
-          sample_extract_mask_coeff(acc + (size_t)r * N, N, nth, tt));
-    }
-    if (tid == 0)
-      o[(size_t)k * N] = Io::narrow(acc[(size_t)k * N + nth]);
-  }
+  sample_extract_many_lut(lwe_out, (uint64_t)out_idx[s], num_samples, num_many_lut,
+                          lut_stride, acc, N, k, N, tid, NTHREADS,
+                          [](uint64_t x) { return Io::narrow(x); });
   __syncthreads(); // the working set is reused by the next sample of this CTA
   } // sample loop
 }

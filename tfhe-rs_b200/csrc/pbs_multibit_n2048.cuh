@@ -316,19 +316,8 @@ pbs_multibit_n2048_k1_kernel(uint64_t *__restrict__ lwe_out,
     acc_s[g * P22_N + 64 * j1 + t + P22_M] = acc_hi[j1];
   }
   __syncthreads();
-  const uint64_t out_len = P22_N + 1;
-  for (uint32_t m = 0; m < num_many_lut; m++) {
-    const uint32_t nth = m * lut_stride;
-    uint64_t *out =
-        lwe_out + ((uint64_t)m * gridDim.x + out_idx[s_idx]) * out_len;
-    for (uint32_t tt = tid; tt < P22_N; tt += 128) {
-      const uint32_t x =
-          tt <= nth ? acc_s[nth - tt] : 0u - acc_s[P22_N + nth - tt];
-      out[tt] = (uint64_t)x << 32;
-    }
-    if (tid == 0)
-      out[P22_N] = (uint64_t)acc_s[P22_N + nth] << 32;
-  }
+  sample_extract_many_lut(lwe_out, out_idx[s_idx], gridDim.x, num_many_lut, lut_stride,
+                          acc_s, P22_N, 1, P22_N, tid, 128, Torus32To64());
 }
 
 // ---------------------------------------------------------------------------
@@ -525,19 +514,8 @@ pbs_multibit_seq_kernel(uint64_t *__restrict__ lwe_out,
     acc_s[g * P22_N + 64 * j1 + t + P22_M] = acc_hi[j1];
   }
   __syncthreads();
-  const uint64_t out_len = P22_N + 1;
-  for (uint32_t m = 0; m < num_many_lut; m++) {
-    const uint32_t nth = m * lut_stride;
-    uint64_t *out =
-        lwe_out + ((uint64_t)m * gridDim.x + out_idx[s_idx]) * out_len;
-    for (uint32_t tt = tid; tt < P22_N; tt += 128) {
-      const uint32_t x =
-          tt <= nth ? acc_s[nth - tt] : 0u - acc_s[P22_N + nth - tt];
-      out[tt] = (uint64_t)x << 32;
-    }
-    if (tid == 0)
-      out[P22_N] = (uint64_t)acc_s[P22_N + nth] << 32;
-  }
+  sample_extract_many_lut(lwe_out, out_idx[s_idx], gridDim.x, num_many_lut, lut_stride,
+                          acc_s, P22_N, 1, P22_N, tid, 128, Torus32To64());
 }
 
 // key conversion into the layout above.  grid = #source polynomials

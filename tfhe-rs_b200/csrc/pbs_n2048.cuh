@@ -132,56 +132,23 @@ pbs_n2048_k1_l1_kernel(uint64_t *__restrict__ lwe_out,
   const uint32_t s = blockIdx.x;
   const uint32_t log_mod = 12;  // log2(2N)
 
-  // ---- prologue: modulus switch (a4/a5) -------------------------------
+  // ---- prologue: modulus switch (a4/a5), acc = LUT * X^{-b_hat} -----------
   const uint64_t *ct = lwe_in + in_idx[s] * (uint64_t)(n + 1);
-  unsigned long long half_sum = 0;
-  long long dbl_sum = 0;
+  CenteredMsSums sums;
   for (uint32_t i = tid; i < n; i += 128) {
     const uint64_t a = ct[i];
     sm.a_hat[i] = (uint16_t)modulus_switch_u64(a, log_mod);
-    if (centered_ms) {
-      int64_t d;
-      half_sum += (unsigned long long)centered_ms_half_error(a, log_mod, &d);
-      dbl_sum += d;
-    }
+    if (centered_ms)
+      sums.add(a, log_mod);
   }
-  if (centered_ms) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      half_sum += __shfl_xor_sync(0xffffffffu, half_sum, off);
-      dbl_sum += __shfl_xor_sync(0xffffffffu, dbl_sum, off);
-    }
-    if ((tid & 31) == 0) {
-      sm.red_half[tid >> 5] = half_sum;
-      sm.red_dbl[tid >> 5] = dbl_sum;
-    }
-  }
+  if (centered_ms)
+    centered_ms_publish_warp(sums, sm.red_half, sm.red_dbl);
   __syncthreads();
-  if (tid == 0) {
-    uint64_t body = ct[n];
-    if (centered_ms) {
-      uint64_t hs = 0;
-      int64_t ds = 0;
-      for (int w = 0; w < 4; w++) {
-        hs += sm.red_half[w];
-        ds += sm.red_dbl[w];
-      }
-      hs -= (uint64_t)(ds / 2);
-      body += hs - ((uint64_t)1 << (63 - log_mod));
-    }
-    sm.b_hat = modulus_switch_u64(body, log_mod);
-  }
+  if (tid == 0)
+    sm.b_hat = ms_b_hat(ct[n], centered_ms, sm.red_half, sm.red_dbl, 4, log_mod);
   __syncthreads();
-
-  // ---- prologue: acc = LUT * X^{-b_hat} ------------------------------
-  {
-    const uint64_t *lut = luts + lut_idx[s] * (uint64_t)(2 * P22_N);
-    const uint32_t b_hat = sm.b_hat;
-    for (uint32_t j = tid; j < 2 * P22_N; j += 128) {
-      const uint32_t r = j >> 11, jj = j & (P22_N - 1);
-      sm.acc[r][jj] = rot_div_coeff(lut + r * P22_N, P22_N, jj, b_hat);
-    }
-  }
+  rotate_lut(&sm.acc[0][0], P22_N, luts + lut_idx[s] * (uint64_t)(2 * P22_N), 2,
+             P22_N, sm.b_hat, tid, 128, SameWord());
 
   // loop-invariant twiddles -> registers
   cplx tw2[3], tw3[15];
@@ -236,15 +203,8 @@ pbs_n2048_k1_l1_kernel(uint64_t *__restrict__ lwe_out,
   __syncthreads();
 
   // ---- epilogue: sample extract (a16), optional many-LUT --------------
-  const uint64_t out_len = P22_N + 1;
-  for (uint32_t m = 0; m < num_many_lut; m++) {
-    const uint32_t nth = m * lut_stride;
-    uint64_t *out = lwe_out + ((uint64_t)m * gridDim.x + out_idx[s]) * out_len;
-    for (uint32_t tt = tid; tt < P22_N; tt += 128)
-      out[tt] = sample_extract_mask_coeff(sm.acc[0], P22_N, nth, tt);
-    if (tid == 0)
-      out[P22_N] = sm.acc[1][nth];
-  }
+  sample_extract_many_lut(lwe_out, out_idx[s], gridDim.x, num_many_lut, lut_stride,
+                          &sm.acc[0][0], P22_N, 1, P22_N, tid, 128, SameWord());
 }
 
 // ---------------------------------------------------------------------------
@@ -474,53 +434,21 @@ pbs_n2048_k1_l1_v3_kernel(uint64_t *__restrict__ lwe_out,
   const uint32_t log_mod = 12;
 
   const uint64_t *ct = lwe_in + in_idx[s] * (uint64_t)(n + 1);
-  unsigned long long half_sum = 0;
-  long long dbl_sum = 0;
+  CenteredMsSums sums;
   for (uint32_t i = tid; i < n; i += 128) {
     const uint64_t a = ct[i];
     sm.a_hat[i] = (uint16_t)modulus_switch_u64(a, log_mod);
-    if (centered_ms) {
-      int64_t d;
-      half_sum += (unsigned long long)centered_ms_half_error(a, log_mod, &d);
-      dbl_sum += d;
-    }
+    if (centered_ms)
+      sums.add(a, log_mod);
   }
-  if (centered_ms) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      half_sum += __shfl_xor_sync(0xffffffffu, half_sum, off);
-      dbl_sum += __shfl_xor_sync(0xffffffffu, dbl_sum, off);
-    }
-    if ((tid & 31) == 0) {
-      sm.red_half[tid >> 5] = half_sum;
-      sm.red_dbl[tid >> 5] = dbl_sum;
-    }
-  }
+  if (centered_ms)
+    centered_ms_publish_warp(sums, sm.red_half, sm.red_dbl);
   __syncthreads();
-  if (tid == 0) {
-    uint64_t body = ct[n];
-    if (centered_ms) {
-      uint64_t hs = 0;
-      int64_t ds = 0;
-      for (int w = 0; w < 4; w++) {
-        hs += sm.red_half[w];
-        ds += sm.red_dbl[w];
-      }
-      hs -= (uint64_t)(ds / 2);
-      body += hs - ((uint64_t)1 << (63 - log_mod));
-    }
-    sm.b_hat = modulus_switch_u64(body, log_mod);
-  }
+  if (tid == 0)
+    sm.b_hat = ms_b_hat(ct[n], centered_ms, sm.red_half, sm.red_dbl, 4, log_mod);
   __syncthreads();
-  {
-    const uint64_t *lut = luts + lut_idx[s] * (uint64_t)(2 * P22_N);
-    const uint32_t b_hat = sm.b_hat;
-    for (uint32_t j = tid; j < 2 * P22_N; j += 128) {
-      const uint32_t r = j >> 11, jj = j & (P22_N - 1);
-      sm.acc[r][jj] =
-          torus64_to_32(rot_div_coeff(lut + r * P22_N, P22_N, jj, b_hat));
-    }
-  }
+  rotate_lut(&sm.acc[0][0], P22_N, luts + lut_idx[s] * (uint64_t)(2 * P22_N), 2,
+             P22_N, sm.b_hat, tid, 128, Torus64To32());
   cplx tw2[3], tw3[15];
 #pragma unroll
   for (int e = 0; e < 3; e++)
@@ -532,19 +460,8 @@ pbs_n2048_k1_l1_v3_kernel(uint64_t *__restrict__ lwe_out,
 
   p22v3_blind_rotate<MAC_MODE, DIG_MODE, X2_MODE>(sm, bsk, g, t, n, base_log, tw2, tw3);
   __syncthreads();
-
-  const uint64_t out_len = P22_N + 1;
-  for (uint32_t m = 0; m < num_many_lut; m++) {
-    const uint32_t nth = m * lut_stride;
-    uint64_t *out = lwe_out + ((uint64_t)m * gridDim.x + out_idx[s]) * out_len;
-    for (uint32_t tt = tid; tt < P22_N; tt += 128) {
-      const uint32_t x = tt <= nth ? sm.acc[0][nth - tt]
-                                   : 0u - sm.acc[0][P22_N + nth - tt];
-      out[tt] = (uint64_t)x << 32;
-    }
-    if (tid == 0)
-      out[P22_N] = (uint64_t)sm.acc[1][nth] << 32;
-  }
+  sample_extract_many_lut(lwe_out, out_idx[s], gridDim.x, num_many_lut, lut_stride,
+                          &sm.acc[0][0], P22_N, 1, P22_N, tid, 128, Torus32To64());
 }
 
 // ---------------------------------------------------------------------------
@@ -643,31 +560,18 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
     mbar_fence_init();
   }
   const uint64_t *ct = lwe_in + in_idx[s] * (uint64_t)(n + 1);
-  unsigned long long half_sum = 0;
-  long long dbl_sum = 0;
+  CenteredMsSums sums;
   if (centered_ms || STAGE_A) {
     for (uint32_t i = tid; i < n; i += 128) {
       const uint64_t a = ct[i];
       if constexpr (STAGE_A)
         sm.a_hat[i] = (uint16_t)modulus_switch_u64(a, log_mod);
-      if (centered_ms) {
-        int64_t d;
-        half_sum += (unsigned long long)centered_ms_half_error(a, log_mod, &d);
-        dbl_sum += d;
-      }
+      if (centered_ms)
+        sums.add(a, log_mod);
     }
   }
-  if (centered_ms) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      half_sum += __shfl_xor_sync(0xffffffffu, half_sum, off);
-      dbl_sum += __shfl_xor_sync(0xffffffffu, dbl_sum, off);
-    }
-    if ((tid & 31) == 0) {
-      sm.red_half[tid >> 5] = half_sum;
-      sm.red_dbl[tid >> 5] = dbl_sum;
-    }
-  }
+  if (centered_ms)
+    centered_ms_publish_warp(sums, sm.red_half, sm.red_dbl);
   __syncthreads();
   auto tma_issue = [&](uint32_t i) {
     if constexpr (KEY_MODE == 2) {
@@ -688,29 +592,11 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
   if (tid == 0) {
     if (KEY_MODE != 1 && n > 0)
       tma_issue(0);
-    uint64_t body = ct[n];
-    if (centered_ms) {
-      uint64_t hs = 0;
-      int64_t ds = 0;
-      for (int w = 0; w < 4; w++) {
-        hs += sm.red_half[w];
-        ds += sm.red_dbl[w];
-      }
-      hs -= (uint64_t)(ds / 2);
-      body += hs - ((uint64_t)1 << (63 - log_mod));
-    }
-    sm.b_hat = modulus_switch_u64(body, log_mod);
+    sm.b_hat = ms_b_hat(ct[n], centered_ms, sm.red_half, sm.red_dbl, 4, log_mod);
   }
   __syncthreads();
-  {
-    const uint64_t *lut = luts + lut_idx[s] * (uint64_t)(2 * P22_N);
-    const uint32_t b_hat = sm.b_hat;
-    for (uint32_t j = tid; j < 2 * P22_N; j += 128) {
-      const uint32_t r = j >> 11, jj = j & (P22_N - 1);
-      sm.acc[r][jj] =
-          torus64_to_32(rot_div_coeff(lut + r * P22_N, P22_N, jj, b_hat));
-    }
-  }
+  rotate_lut(&sm.acc[0][0], P22_ACC_STRIDE, luts + lut_idx[s] * (uint64_t)(2 * P22_N),
+             2, P22_N, sm.b_hat, tid, 128, Torus64To32());
   cplx tw2[3], tw3[15];
 #pragma unroll
   for (int e = 0; e < 3; e++)
@@ -896,19 +782,9 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
     }
   }
   __syncthreads();
-
-  const uint64_t out_len = P22_N + 1;
-  for (uint32_t m = 0; m < num_many_lut; m++) {
-    const uint32_t nth = m * lut_stride;
-    uint64_t *out = lwe_out + ((uint64_t)m * gridDim.x + out_idx[s]) * out_len;
-    for (uint32_t tt = tid; tt < P22_N; tt += 128) {
-      const uint32_t x = tt <= nth ? sm.acc[0][nth - tt]
-                                   : 0u - sm.acc[0][P22_N + nth - tt];
-      out[tt] = (uint64_t)x << 32;
-    }
-    if (tid == 0)
-      out[P22_N] = (uint64_t)sm.acc[1][nth] << 32;
-  }
+  sample_extract_many_lut(lwe_out, out_idx[s], gridDim.x, num_many_lut, lut_stride,
+                          &sm.acc[0][0], P22_ACC_STRIDE, 1, P22_N, tid, 128,
+                          Torus32To64());
 }
 
 // ---------------------------------------------------------------------------

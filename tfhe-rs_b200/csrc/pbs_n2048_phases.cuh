@@ -92,21 +92,32 @@ B200_HD void p22_acc_update(uint64_t *acc_g, int t, const cplx v[16]) {
   }
 }
 
+// ===========================================================================
+// The integer stages either side of every blind rotation, shared by all PBS
+// kernels and their CPU replays: the modulus switch of the input LWE (standard
+// or centered mean), acc = LUT * X^{-b_hat}, and the many-LUT sample extract.
+// ===========================================================================
+
 // LUT * X^{-b_hat} coefficient j (polynomial_wrapping_monic_monomial_div)
-B200_HD uint64_t rot_div_coeff(const uint64_t *lut, uint32_t N, uint32_t j,
-                               uint32_t b_hat) {
+template <typename Word>
+B200_HD Word rot_div_coeff(const Word *lut, uint32_t N, uint32_t j,
+                           uint32_t b_hat) {
   const uint32_t d = b_hat & (N - 1);
   const bool neg0 = b_hat >= N;
   const uint32_t s = j + d;
   const bool wrap = s >= N;
-  const uint64_t x = lut[wrap ? s - N : s];
-  return (neg0 != wrap) ? (uint64_t)0 - x : x;
+  const Word x = lut[wrap ? s - N : s];
+  return (neg0 != wrap) ? (Word)0 - x : x;
 }
 
-// modulus switch to 2N (fft_impl/common.rs:10-23)
+// modulus switch to 2^log_modulus, rounded (fft_impl/common.rs:10-23)
+B200_HD uint64_t modulus_switch_full(uint64_t x, uint32_t log_modulus) {
+  return (x + ((uint64_t)1 << (63 - log_modulus))) >> (64 - log_modulus);
+}
+
+// the same, to 2N <= 2^32
 B200_HD uint32_t modulus_switch_u64(uint64_t x, uint32_t log_modulus) {
-  return (uint32_t)((x + ((uint64_t)1 << (63 - log_modulus))) >>
-                    (64 - log_modulus));
+  return (uint32_t)modulus_switch_full(x, log_modulus);
 }
 
 // per-element terms of the centered-mean body correction
@@ -131,6 +142,126 @@ B200_HD Word sample_extract_mask_coeff(const Poly &A, uint32_t N, uint32_t nth,
                                        uint32_t t) {
   return t <= nth ? A[nth - t] : (Word)0 - A[N + nth - t];
 }
+
+// A thread's share of the two sums of the centered-mean correction, over the
+// mask words it switches.  Integer sums: every grouping gives the same words.
+struct CenteredMsSums {
+  unsigned long long half = 0;
+  long long dbl = 0;
+  B200_HD void add(uint64_t a, uint32_t log_modulus) {
+    int64_t d;
+    half += (unsigned long long)centered_ms_half_error(a, log_modulus, &d);
+    dbl += d;
+  }
+};
+
+// The body plus the centered-mean correction.  The sums of the whole mask
+// arrive as `nslots` partial sums (one per warp, or a single shared total):
+// ds / 2 truncates toward zero, so it is taken once, on the total.
+B200_HD uint64_t centered_ms_body(uint64_t body, const unsigned long long *half,
+                                  const long long *dbl, int nslots,
+                                  uint32_t log_modulus) {
+  uint64_t hs = 0;
+  int64_t ds = 0;
+  for (int w = 0; w < nslots; w++) {
+    hs += half[w];
+    ds += dbl[w];
+  }
+  return body + (hs - (uint64_t)(ds / 2)) - ((uint64_t)1 << (63 - log_modulus));
+}
+
+// b_hat: the body switched to 2N, with or without the centered correction
+B200_HD uint32_t ms_b_hat(uint64_t body, bool centered,
+                          const unsigned long long *half, const long long *dbl,
+                          int nslots, uint32_t log_modulus) {
+  if (centered)
+    body = centered_ms_body(body, half, dbl, nslots, log_modulus);
+  return modulus_switch_u64(body, log_modulus);
+}
+
+#if defined(__CUDACC__)
+// Publish step of the warp form of the sum reduction (thread counts that are
+// multiples of 32): each warp's total goes to slot threadIdx.x / 32.  After
+// the caller's barrier one thread reads the slots (nslots = warps).
+__device__ __forceinline__ void centered_ms_publish_warp(CenteredMsSums s,
+                                                         unsigned long long *half,
+                                                         long long *dbl) {
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    s.half += __shfl_xor_sync(0xffffffffu, s.half, off);
+    s.dbl += __shfl_xor_sync(0xffffffffu, s.dbl, off);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    half[threadIdx.x >> 5] = s.half;
+    dbl[threadIdx.x >> 5] = s.dbl;
+  }
+}
+
+// Publish step of the shared-memory form (groups that are not warp multiples,
+// or several LWEs per CTA): atomic adds into one slot, zeroed before an
+// earlier barrier.  After the caller's barrier nslots = 1.
+__device__ __forceinline__ void centered_ms_publish_atomic(const CenteredMsSums &s,
+                                                           unsigned long long *half,
+                                                           long long *dbl) {
+  atomicAdd(half, s.half);
+  atomicAdd(reinterpret_cast<unsigned long long *>(dbl), (unsigned long long)s.dbl);
+}
+#endif
+
+// acc = LUT * X^{-b_hat} for `rows` polynomials of N coefficients: flat
+// coefficient j = r N + c for j = first, first + step, ...; acc rows are
+// acc_stride words apart; cvt maps the LUT word to the accumulator word.
+template <typename Acc, typename Word, typename Cvt>
+B200_HD void rotate_lut(Acc *acc, uint32_t acc_stride, const Word *lut,
+                        uint32_t rows, uint32_t N, uint32_t b_hat,
+                        uint32_t first, uint32_t step, Cvt cvt) {
+  for (uint32_t j = first; j < rows * N; j += step) {
+    const uint32_t r = j / N, c = j % N;
+    (acc + (size_t)r * acc_stride)[c] = cvt(rot_div_coeff(lut + (size_t)r * N, N, c, b_hat));
+  }
+}
+
+// The LWE extracted at coefficient nth of the GLWE in acc (k mask rows, then
+// the body row, acc_stride words apart): mask word w = r N + t for
+// w = first, first + step, ..., and the body, word k N, by the thread with
+// first = 0; cvt maps the accumulator word to the output word.
+template <typename Out, typename Acc, typename Cvt>
+B200_HD void sample_extract_lwe(Out *out, const Acc *acc, uint32_t acc_stride,
+                                uint32_t k, uint32_t N, uint32_t nth,
+                                uint32_t first, uint32_t step, Cvt cvt) {
+  for (uint32_t w = first; w < k * N; w += step) {
+    // r = 0 spelled out for k = 1: the compiler does not derive it from
+    // w < N, and the row split changed the register allocation of the
+    // multi-bit N = 2048 kernels
+    const uint32_t r = k > 1 ? w / N : 0, t = w - r * N;
+    out[w] = cvt(sample_extract_mask_coeff(acc + (size_t)r * acc_stride, N, nth, t));
+  }
+  if (first == 0)
+    out[(size_t)k * N] = cvt(acc[(size_t)k * acc_stride + nth]);
+}
+
+// Many-LUT output layout: LUT m of the sample goes to coefficient
+// nth = m * lut_stride and to LWE m * batch + out_idx of lwe_out.
+template <typename Out, typename Acc, typename Cvt>
+B200_HD void sample_extract_many_lut(Out *lwe_out, uint64_t out_idx, uint64_t batch,
+                                     uint32_t num_many_lut, uint32_t lut_stride,
+                                     const Acc *acc, uint32_t acc_stride,
+                                     uint32_t k, uint32_t N, uint32_t first,
+                                     uint32_t step, Cvt cvt) {
+  const uint64_t out_len = (uint64_t)k * N + 1;
+  for (uint32_t m = 0; m < num_many_lut; m++)
+    sample_extract_lwe(lwe_out + ((uint64_t)m * batch + out_idx) * out_len, acc,
+                       acc_stride, k, N, m * lut_stride, first, step, cvt);
+}
+
+// word conversions of the two helpers above
+struct SameWord {
+  template <typename T> B200_HD T operator()(T x) const { return x; }
+};
+// the 32-bit accumulators keep bits 63..32 of the torus word
+struct Torus32To64 {
+  B200_HD uint64_t operator()(uint32_t x) const { return (uint64_t)x << 32; }
+};
 
 // ===========================================================================
 // v2 phases: 32-bit running accumulator.
@@ -180,6 +311,9 @@ B200_HD void p22v2_acc_update(uint32_t *acc_g, int t, const cplx v[16]) {
 B200_HD uint32_t torus64_to_32(uint64_t x) {
   return (uint32_t)((x + 0x80000000ull) >> 32);
 }
+struct Torus64To32 {
+  B200_HD uint32_t operator()(uint64_t x) const { return torus64_to_32(x); }
+};
 
 // MAC with explicit software prefetch: the 16 "own-row" key values are loaded
 // by the caller before the last forward pass (their L2 latency hides behind the

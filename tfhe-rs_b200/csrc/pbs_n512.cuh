@@ -179,35 +179,21 @@ pbs_n512_kernel(uint64_t *__restrict__ lwe_out,
   }
   __syncthreads();
   {
-    unsigned long long half_sum = 0;
-    long long dbl_sum = 0;
+    CenteredMsSums sums;
     for (uint32_t i = tl; i < n; i += TPL) {
       const uint64_t a = ct[i];
       sm.a_hat[lw][i] = (uint16_t)modulus_switch_u64(a, log_mod);
-      if (centered_ms) {
-        int64_t dd;
-        half_sum += (unsigned long long)centered_ms_half_error(a, log_mod, &dd);
-        dbl_sum += dd;
-      }
+      if (centered_ms)
+        sums.add(a, log_mod);
     }
     // per-LWE reduction through shared memory (TPL is not a warp multiple)
-    if (centered_ms) {
-      atomicAdd(&sm.red_half[lw][0], half_sum);
-      atomicAdd(reinterpret_cast<unsigned long long *>(&sm.red_dbl[lw][0]),
-                (unsigned long long)dbl_sum);
-    }
+    if (centered_ms)
+      centered_ms_publish_atomic(sums, &sm.red_half[lw][0], &sm.red_dbl[lw][0]);
   }
   __syncthreads();
-  if (tl == 0) {
-    uint64_t body = ct[n];
-    if (centered_ms) {
-      uint64_t hs = sm.red_half[lw][0];
-      const int64_t ds = sm.red_dbl[lw][0];
-      hs -= (uint64_t)(ds / 2);
-      body += hs - ((uint64_t)1 << (63 - log_mod));
-    }
-    sm.b_hat[lw] = modulus_switch_u64(body, log_mod);
-  }
+  if (tl == 0)
+    sm.b_hat[lw] = ms_b_hat(ct[n], centered_ms, &sm.red_half[lw][0],
+                            &sm.red_dbl[lw][0], 1, log_mod);
   __syncthreads();
   // ---- prologue: acc = LUT * X^{-b_hat} ------------------------------------
   {

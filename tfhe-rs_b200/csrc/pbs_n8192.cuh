@@ -211,44 +211,22 @@ pbs_n8192_k1_l2_kernel(uint64_t *__restrict__ lwe_out,
     }
     __syncthreads();
     {
-      unsigned long long half_sum = 0;
-      long long dbl_sum = 0;
+      CenteredMsSums sums;
       for (uint32_t i = t; i < n; i += 256) {
         const uint64_t a = ct[i];
         sm.a_hat[i] = (uint16_t)modulus_switch_u64(a, log_mod);
-        if (centered_ms) {
-          int64_t dd;
-          half_sum += (unsigned long long)centered_ms_half_error(a, log_mod, &dd);
-          dbl_sum += dd;
-        }
+        if (centered_ms)
+          sums.add(a, log_mod);
       }
-      if (centered_ms) {
-        atomicAdd(&sm.red_half, half_sum);
-        atomicAdd(reinterpret_cast<unsigned long long *>(&sm.red_dbl),
-                  (unsigned long long)dbl_sum);
-      }
+      if (centered_ms)
+        centered_ms_publish_atomic(sums, &sm.red_half, &sm.red_dbl);
     }
     __syncthreads();
-    if (t == 0) {
-      uint64_t body = ct[n];
-      if (centered_ms) {
-        uint64_t hs = sm.red_half;
-        const int64_t ds = sm.red_dbl;
-        hs -= (uint64_t)(ds / 2);
-        body += hs - ((uint64_t)1 << (63 - log_mod));
-      }
-      sm.b_hat = modulus_switch_u64(body, log_mod);
-    }
+    if (t == 0)
+      sm.b_hat = ms_b_hat(ct[n], centered_ms, &sm.red_half, &sm.red_dbl, 1, log_mod);
     __syncthreads();
-    {
-      const uint64_t *lut = luts + lut_idx[s] * (uint64_t)(2 * P8K_N);
-      const uint32_t b_hat = sm.b_hat;
-      for (uint32_t j = t; j < 2 * P8K_N; j += 256) {
-        const uint32_t r = j >> 13, jj = j & (P8K_N - 1);
-        sm.acc[r][jj] =
-            torus64_to_32(rot_div_coeff(lut + r * P8K_N, P8K_N, jj, b_hat));
-      }
-    }
+    rotate_lut(&sm.acc[0][0], P8K_N, luts + lut_idx[s] * (uint64_t)(2 * P8K_N), 2,
+               P8K_N, sm.b_hat, t, 256, Torus64To32());
     __syncthreads();
 
     // ---- blind rotation ---------------------------------------------------------
@@ -314,18 +292,8 @@ pbs_n8192_k1_l2_kernel(uint64_t *__restrict__ lwe_out,
     __syncthreads();
 
     // ---- epilogue: sample extract, optional many-LUT ---------------------------
-    const uint64_t out_len = (uint64_t)P8K_N + 1;
-    for (uint32_t m = 0; m < num_many_lut; m++) {
-      const uint32_t nth = m * lut_stride;
-      uint64_t *o = lwe_out + ((uint64_t)m * num_samples + out_idx[s]) * out_len;
-      for (uint32_t tt = t; tt < P8K_N; tt += 256) {
-        const uint32_t x = tt <= nth ? sm.acc[0][nth - tt]
-                                     : 0u - sm.acc[0][P8K_N + nth - tt];
-        o[tt] = (uint64_t)x << 32;
-      }
-      if (t == 0)
-        o[P8K_N] = (uint64_t)sm.acc[1][nth] << 32;
-    }
+    sample_extract_many_lut(lwe_out, out_idx[s], num_samples, num_many_lut, lut_stride,
+                            &sm.acc[0][0], P8K_N, 1, P8K_N, t, 256, Torus32To64());
     __syncthreads(); // the working set is reused by the next sample
   }
 }
@@ -485,22 +453,15 @@ pbs_n8192_k1_l2_v2_kernel(uint64_t *__restrict__ lwe_out,
     }
     __syncthreads();
     {
-      unsigned long long half_sum = 0;
-      long long dbl_sum = 0;
+      CenteredMsSums sums;
       for (uint32_t i = t; i < n; i += 256) {
         const uint64_t a = ct[i];
         sm.a_hat[i] = (uint16_t)modulus_switch_u64(a, log_mod);
-        if (centered_ms) {
-          int64_t dd;
-          half_sum += (unsigned long long)centered_ms_half_error(a, log_mod, &dd);
-          dbl_sum += dd;
-        }
+        if (centered_ms)
+          sums.add(a, log_mod);
       }
-      if (centered_ms) {
-        atomicAdd(&sm.red_half, half_sum);
-        atomicAdd(reinterpret_cast<unsigned long long *>(&sm.red_dbl),
-                  (unsigned long long)dbl_sum);
-      }
+      if (centered_ms)
+        centered_ms_publish_atomic(sums, &sm.red_half, &sm.red_dbl);
     }
     __syncthreads();
     if (t == 0) {
@@ -511,25 +472,11 @@ pbs_n8192_k1_l2_v2_kernel(uint64_t *__restrict__ lwe_out,
         p_step++;
       for (int f = 0; f < P8K_SLOTS; f++)
         produce();
-      uint64_t body = ct[n];
-      if (centered_ms) {
-        uint64_t hs = sm.red_half;
-        const int64_t ds = sm.red_dbl;
-        hs -= (uint64_t)(ds / 2);
-        body += hs - ((uint64_t)1 << (63 - log_mod));
-      }
-      sm.b_hat = modulus_switch_u64(body, log_mod);
+      sm.b_hat = ms_b_hat(ct[n], centered_ms, &sm.red_half, &sm.red_dbl, 1, log_mod);
     }
     __syncthreads();
-    {
-      const uint64_t *lut = luts + lut_idx[s] * (uint64_t)(2 * P8K_N);
-      const uint32_t b_hat = sm.b_hat;
-      for (uint32_t j = t; j < 2 * P8K_N; j += 256) {
-        const uint32_t r = j >> 13, jj = j & (P8K_N - 1);
-        sm.acc[r][jj] =
-            torus64_to_32(rot_div_coeff(lut + r * P8K_N, P8K_N, jj, b_hat));
-      }
-    }
+    rotate_lut(&sm.acc[0][0], P8K_N, luts + lut_idx[s] * (uint64_t)(2 * P8K_N), 2,
+               P8K_N, sm.b_hat, t, 256, Torus64To32());
     __syncthreads();
 
     // ---- blind rotation ---------------------------------------------------------
@@ -611,18 +558,8 @@ pbs_n8192_k1_l2_v2_kernel(uint64_t *__restrict__ lwe_out,
     __syncthreads();
 
     // ---- epilogue: sample extract, optional many-LUT ---------------------------
-    const uint64_t out_len = (uint64_t)P8K_N + 1;
-    for (uint32_t m = 0; m < num_many_lut; m++) {
-      const uint32_t nth = m * lut_stride;
-      uint64_t *o = lwe_out + ((uint64_t)m * num_samples + out_idx[s]) * out_len;
-      for (uint32_t tt = t; tt < P8K_N; tt += 256) {
-        const uint32_t x = tt <= nth ? sm.acc[0][nth - tt]
-                                     : 0u - sm.acc[0][P8K_N + nth - tt];
-        o[tt] = (uint64_t)x << 32;
-      }
-      if (t == 0)
-        o[P8K_N] = (uint64_t)sm.acc[1][nth] << 32;
-    }
+    sample_extract_many_lut(lwe_out, out_idx[s], num_samples, num_many_lut, lut_stride,
+                            &sm.acc[0][0], P8K_N, 1, P8K_N, t, 256, Torus32To64());
     __syncthreads(); // the working set is reused by the next sample
   }
 }
