@@ -2,9 +2,10 @@
 of the exchange-1 buffer (x2m_*, csrc/x2_smem.cuh) instead of half-warp
 shuffles (x2h_*, csrc/x2_shfl.cuh).
 
-CPU: x2m_* leaves exactly the registers x2h_* leaves on all 32 lanes, every
-quarter-warp access of its slot map is bank-conflict free, and a whole PBS
-replayed with it is word-identical to the lane-pair replay with shuffles.
+CPU (tests/emu/emu_lanepair.cpp): x2m_* leaves exactly the registers x2h_*
+leaves on all 32 lanes, every quarter-warp access of its slot map is
+bank-conflict free, and a whole PBS replayed with it is word-identical to the
+lane-pair replay with shuffles.
 GPU: the two lane-pair instances and the round-1 kernel agree word for word on
 a PARAM_MESSAGE_2_CARRY_2 key, and the automatic two-CTA route runs the
 instance with exchange 2 through shared memory."""
@@ -23,19 +24,18 @@ NAMES = {X2M: "n2048_v6<2,true,2,1>", X2H: "n2048_v6<2,true,2,1,0>", ROUND1: "n2
 
 @pytest.fixture(scope="module")
 def emus(tmp_path_factory):
-    """(lane-pair replay with shuffles, lane-pair replay through shared memory,
-    emulator of the other layouts for the key conversion), all built without
-    floating-point contraction so that word identity is a question of which
-    operations run in which order."""
+    """(lane-pair replay with either exchange 2, emulator of the other layouts
+    for the key conversion), both built without floating-point contraction so
+    that word identity is a question of which operations run in which order."""
     d = tmp_path_factory.mktemp("emu_x2m")
     gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
     libs = []
-    for src in ("emu_lanepair.cpp", "emu_x2m.cpp", "emu_p22.cpp"):
+    for src in ("emu_lanepair.cpp", "emu_p22.cpp"):
         out = str(d / src.replace(".cpp", ".so"))
         subprocess.check_call([gxx, "-O2", "-mavx2", "-mfma", "-ffp-contract=off", "-std=c++17", "-fPIC", "-shared",
                                "-w", "-x", "c++", os.path.join(HERE, "emu", src), "-o", out])
         libs.append(C.CDLL(out))
-    libs[1].emu_x2m_register_check.argtypes = [C.c_uint64]
+    libs[0].emu_x2m_register_check.argtypes = [C.c_uint64]
     return libs
 
 
@@ -51,15 +51,15 @@ def _p22(oracle, n):
 @pytest.mark.parametrize("seed", [1, 2, 0xC0FFEE])
 def test_x2m_reproduces_x2h_register_for_register(emus, seed):
     """Forward and inverse, all 32 lanes x 16 registers, bit for bit."""
-    assert emus[1].emu_x2m_register_check(seed) == 0
+    assert emus[0].emu_x2m_register_check(seed) == 0
 
 
 def test_x2m_slot_map_is_bank_conflict_free(emus):
     """Both access sides of both directions hit 8 distinct 16-byte bank groups
     per quarter-warp; the unswizzled map 16 i + b would be an 8-way conflict on
     the pass-3 side, which the audit sees."""
-    assert emus[1].emu_x2m_conflict_audit(1) == 1
-    assert emus[1].emu_x2m_conflict_audit(0) == 8
+    assert emus[0].emu_x2m_conflict_audit(1) == 1
+    assert emus[0].emu_x2m_conflict_audit(0) == 8
 
 
 @pytest.mark.parametrize("n,centered,many", [(1, True, 1), (16, True, 2), (48, False, 2)])
@@ -69,7 +69,7 @@ def test_x2m_replay_is_word_identical(oracle, keyset, emus, n, centered, many):
     P = _p22(oracle, n)
     keys = keyset(P, seed=31 + n, with_ksk=False)
     bskf = np.empty(P.n * 4 * 1024 * 2)
-    lp, x2m, emu = emus
+    lp, emu = emus
     emu.emu_bsk_convert_p22(_vp(keys.bsk), P.n, _vp(bskf))
     msgs = np.arange(6) % 16
     cts = oracle.lwe_encrypt_batch(oracle.Rng(5 + n), keys.lwe_sk, msgs.astype(np.uint64) * np.uint64(P.delta), 45)
@@ -79,7 +79,7 @@ def test_x2m_replay_is_word_identical(oracle, keyset, emus, n, centered, many):
         cts[1, 3] = 0
     lut = oracle.make_lut(P, [(7 * i + 2) % 16 for i in range(16)])
     outs = []
-    for fn in (lp.emu_pbs_p22_lanepair, x2m.emu_pbs_p22_lanepair_x2m):
+    for fn in (lp.emu_pbs_p22_lanepair, lp.emu_pbs_p22_lanepair_x2m):
         out = np.zeros((many, len(cts), 2049), dtype=np.uint64)
         for s in range(len(cts)):
             fn(_vp(bskf), _vp(lut), _vp(np.ascontiguousarray(cts[s])), P.n, P.pbs_base_log, int(centered), many, 3,

@@ -17,6 +17,7 @@
 //     32 KiB contiguous block per (GGSW, column) per step, pre-permuted at
 //     key-conversion time so that lane t reads element t.
 #pragma once
+#include "pbs_n2048_lanepair.cuh"
 #include "pbs_n2048_phases.cuh"
 #include "tma_bulk.cuh"
 #include "x2_shfl.cuh"
@@ -99,11 +100,6 @@ __device__ __forceinline__ void spec_ready_arrive(int g) {
 }
 __device__ __forceinline__ void spec_ready_wait(int g) {
   asm volatile("bar.sync %0, 128;" ::"r"(9 + g) : "memory");
-}
-
-__device__ __forceinline__ cplx ldcg_cplx(const cplx *p) {
-  const double2 v = __ldcg(reinterpret_cast<const double2 *>(p));
-  return cmake(v.x, v.y);
 }
 
 struct LdcgLoader {
@@ -487,10 +483,6 @@ pbs_n2048_k1_l1_v3_kernel(uint64_t *__restrict__ lwe_out,
 // staged in shared memory (2 KiB) -- otherwise step i recomputes a_hat[i] from
 // the input LWE word, loaded one step ahead: with the 64 KiB ring the 2 KiB
 // would push the CTA over half an SM's shared memory.
-// The rows of acc are 16 words apart modulo the 32 banks: in the lane-pair
-// layout a warp reads and writes the same 16 coefficients of both polynomials,
-// and the two halves then hit disjoint banks.
-constexpr int P22_ACC_STRIDE = P22_N + 16;
 template <int RING, bool STAGE_A>
 struct P22SmemV6 {
   cplx xa[2][P22_M];        // 32 KiB  exchange 1 / spectrum share
@@ -513,6 +505,68 @@ static_assert(sizeof(P22SmemV6<2, true>) <= 115712, "v6 hybrid must fit two CTAs
 __constant__ uint32_t c_p22_stagger;
 __device__ uint32_t g_p22_sm_arrivals[512];
 
+// Thread 0: the other-row key blocks of step i into the ring (KEY_MODE 2).
+__device__ __forceinline__ void p22_ring_issue(cplx *ring, unsigned long long *bar,
+                                               const cplx *bsk, uint32_t i) {
+  mbar_arrive_expect_tx(bar, P22_RING_BYTES);
+  tma_bulk_g2s(ring, p22_ring_src(bsk, i), P22_RING_BYTES, bar);
+}
+
+// What p22_lanepair_loop runs between its phases: nothing in the kernel; the
+// phase-clock tool passes a probe that reads the clock.
+struct P22NoProbe {
+  __device__ __forceinline__ void begin() {}
+  __device__ __forceinline__ void lap(int) {}
+};
+
+// The blind rotation of the lane-pair layout (pbs_n2048_lanepair.cuh): the
+// pieces of each CMUX step in order, with the barriers, the warp exchanges and
+// the key wait between them.  The MAC takes the other polynomial's value from
+// lane l ^ 16 with one shuffle: no spectrum store, no barrier between the
+// polynomials before or after it.  Exchange 2 goes through this warp's rows of
+// xa[g] (X2 = 1, x2m_*) or stays inside each half-warp as shuffles (X2 = 0,
+// x2h_*).  The values and the order of every operation are those of the other
+// v6 instances, so the results are bit-identical.  Expects the ring copy of
+// step 0 issued and the accumulator, a_hat and the barrier set up.
+template <int X2, typename Probe>
+__device__ __forceinline__ void
+p22_lanepair_loop(P22SmemV6<2, true> &sm, const cplx *bsk, uint32_t n,
+                  uint32_t base_log, const cplx *tw2, const cplx *tw3, Probe &probe) {
+  const P22LanePair lp(threadIdx.x, sm.acc, sm.xa, sm.ring, bsk, c_fft1024_pass1, tw2, tw3);
+  uint32_t own[32];
+  lp.own_init(own);
+  uint32_t a_next = n > 0 ? sm.a_hat[0] : 0;
+  for (uint32_t i = 0; i < n; i++) {
+    const uint32_t a = a_next; // read a step ahead: every address of the step hangs on it
+    a_next = sm.a_hat[i + 1];  // a_hat has 8 words of padding
+    cplx v[16];
+    probe.begin();
+    lp.digits(a, base_log, own, v);                                     probe.lap(0);
+    lp.fwd_pass1(v);                                                    probe.lap(1);
+    lp.x1_fwd_store(v); __syncthreads(); lp.x1_fwd_load(v);             probe.lap(2);
+    lp.fwd_pass2(v);                                                    probe.lap(3);
+    if constexpr (X2 == 1) x2m_fwd(lp.x2_rows, v); else x2h_fwd(v);     probe.lap(4);
+    lp.fwd_pass3(v);                                                    probe.lap(5);
+    cplx b_own[16];
+    lp.own_row_load(i, b_own); mbar_wait_parity(&sm.bar, i & 1u);       probe.lap(6);
+    lp.mac(v, b_own, [](int, cplx x) { return shfl_xor_cplx(x, 16); }); probe.lap(7);
+    lp.inv_pass3(v);                                                    probe.lap(8);
+    if constexpr (X2 == 1) x2m_inv(lp.x2_rows, v); else x2h_inv(v);     probe.lap(9);
+    lp.inv_pass2(v);                                                    probe.lap(10);
+    // the forward exchange-1 loads (or the exchange-2 loads) of this warp read
+    // the same slots (rows 4 w .. 4 w + 3 of xa[g]); no other warp touches them
+    // in between
+    __syncwarp();
+    lp.x1_inv_store(v);
+    __syncthreads();
+    if (threadIdx.x == 0 && i + 1 < n)
+      p22_ring_issue(&sm.ring[0][0], &sm.bar, bsk, i + 1); // every warp is past its MAC
+    lp.x1_inv_load(v);                                                  probe.lap(11);
+    lp.inv_pass1(v);                                                    probe.lap(12);
+    lp.acc_update(v, own); __syncthreads();                             probe.lap(13);
+  }
+}
+
 // KEY_MODE 0: key block through the TMA ring; 1: v3's register prefetch
 // (own row after the last forward pass, other row after the own products) --
 // the A/B partner that isolates the effect of the ring; 2: own row through
@@ -533,13 +587,13 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
                           uint32_t lut_stride, int centered_ms) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   constexpr int RING = KEY_MODE == 0 ? 4 : KEY_MODE == 2 ? 2 : 1;
-  // The shipped two-CTA instance runs the lane-pair layout (see the loop).
+  // The shipped two-CTA instance runs the lane-pair layout (p22_lanepair_loop).
   constexpr bool LANE_PAIR = KEY_MODE == 2 && STAGE_A && CVT == 2 && SPLIT_POST == 1;
   using Smem = P22SmemV6<RING, STAGE_A>;
   Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
   const int tid = threadIdx.x;
-  const int g = LANE_PAIR ? (tid >> 4) & 1 : tid >> 6;
-  const int t = LANE_PAIR ? ((tid >> 5) << 4) | (tid & 15) : tid & 63;
+  const int g = LANE_PAIR ? p22lp_g(tid) : tid >> 6;
+  const int t = LANE_PAIR ? p22lp_t(tid) : tid & 63;
   const uint32_t s = blockIdx.x;
   const uint32_t log_mod = 12;
 
@@ -575,11 +629,7 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
   __syncthreads();
   auto tma_issue = [&](uint32_t i) {
     if constexpr (KEY_MODE == 2) {
-      // other rows only: blocks 2c + r = 1 (column 0, row 1) and 2 (column 1,
-      // row 0) are adjacent -> one 32 KiB copy
-      mbar_arrive_expect_tx(&sm.bar, 2u * P22_M * (uint32_t)sizeof(cplx));
-      tma_bulk_g2s(&sm.ring[0][0], bsk + (size_t)i * (4 * P22_M) + P22_M,
-                   2u * P22_M * (uint32_t)sizeof(cplx), &sm.bar);
+      p22_ring_issue(&sm.ring[0][0], &sm.bar, bsk, i); // other rows only
     } else {
       mbar_arrive_expect_tx(&sm.bar, 4u * P22_M * (uint32_t)sizeof(cplx));
 #pragma unroll
@@ -606,77 +656,23 @@ pbs_n2048_k1_l1_v6_kernel(uint64_t *__restrict__ lwe_out,
     tw3[e] = tables->pass3[t][e];
   __syncthreads();
 
-  uint32_t *acc_g = sm.acc[g];
-  cplx *xa_g = sm.xa[g];
-  [[maybe_unused]] const cplx *xa_other = sm.xa[1 - g];
-  // ring slot of block 2c + r: RING = 4 -> 2c + r; RING = 2 -> blocks 1, 2 at 0, 1
-  [[maybe_unused]] const cplx *k_own = &sm.ring[RING == 4 ? 2 * g + g : 0][0];
-  const cplx *k_oth = &sm.ring[RING == 4 ? 2 * g + (1 - g) : RING == 2 ? g : 0][0];
-  const cplx *bsk_own = bsk + (size_t)g * (2 * P22_M) + (size_t)g * P22_M + t;
-  [[maybe_unused]] const cplx *bsk_oth =
-      bsk + (size_t)g * (2 * P22_M) + (size_t)(1 - g) * P22_M;
-  uint32_t own[32];
-  p22v4_own_init(acc_g, t, own);
-  [[maybe_unused]] uint64_t ct_next = (!STAGE_A && n > 0) ? ct[0] : 0;
-  [[maybe_unused]] uint32_t a_next = (STAGE_A && n > 0) ? sm.a_hat[0] : 0;
   if constexpr (LANE_PAIR) {
-    // Lane-pair layout: lane l of warp w runs thread t = 16 w + (l & 15) of
-    // polynomial l >> 4, so lanes l and l ^ 16 hold the same spectrum slots
-    // 16 t + b of the two polynomials after the forward transform.  The MAC
-    // takes the other polynomial's value with one shuffle: no spectrum store,
-    // no barrier between the polynomials before or after it.  Exchange 1 goes
-    // through xa[g] (x1h_*); exchange 2 goes through this warp's rows of the
-    // same buffer (X2 = 1, x2m_*: they belong to the warp from x1h_load_p2 to
-    // x1h_store_p2) or stays inside each half-warp as shuffles (X2 = 0,
-    // x2h_*).  The values and the order of every operation are those of the
-    // other instances, so the results are bit-identical.
-    [[maybe_unused]] cplx *x2_rows = xa_g + 256 * (tid >> 5);
-    for (uint32_t i = 0; i < n; i++) {
-      const uint32_t a = a_next; // read a step ahead: every address of the step hangs on it
-      a_next = sm.a_hat[i + 1];  // a_hat has 8 words of padding
-      cplx v[16];
-      p22v4_load_digits<CVT>(acc_g, t, a, base_log, own, v);
-      radix16_fwd(v, c_fft1024_pass1);
-      x1h_store_p1(xa_g, t, v);
-      __syncthreads();
-      x1h_load_p2(xa_g, t, v);
-      pass2_fwd(v, tw2);
-      if constexpr (X2 == 1)
-        x2m_fwd(x2_rows, v);
-      else
-        x2h_fwd(v);
-      radix16_fwd(v, tw3);
-      const size_t step = (size_t)i * (4 * P22_M);
-      cplx b_own[16];
-#pragma unroll
-      for (int b = 0; b < 16; b++)
-        b_own[b] = ldcg_cplx(bsk_own + step + b * 64);
-      mbar_wait_parity(&sm.bar, i & 1u);
-#pragma unroll
-      for (int b = 0; b < 16; b++) {
-        const cplx o = shfl_xor_cplx(v[b], 16);
-        v[b] = cfma(o, k_oth[b * 64 + t], cmul(v[b], b_own[b]));
-      }
-      radix16_inv(v, tw3);
-      if constexpr (X2 == 1)
-        x2m_inv(x2_rows, v);
-      else
-        x2h_inv(v);
-      pass2_inv(v, tw2);
-      // the forward exchange-1 loads (or the exchange-2 loads) of this warp
-      // read the same slots (rows 4 w .. 4 w + 3 of xa[g]); no other warp
-      // touches them in between
-      __syncwarp();
-      x1h_store_p2(xa_g, t, v);
-      __syncthreads();
-      if (tid == 0 && i + 1 < n)
-        tma_issue(i + 1); // every warp is past its MAC: the slot is free
-      x1h_load_p1(xa_g, t, v);
-      radix16_inv(v, c_fft1024_pass1);
-      p22v4_acc_update(acc_g, t, v, own);
-      __syncthreads();
-    }
+    P22NoProbe probe;
+    p22_lanepair_loop<X2>(sm, bsk, n, base_log, tw2, tw3, probe);
   } else {
+    uint32_t *acc_g = sm.acc[g];
+    cplx *xa_g = sm.xa[g];
+    [[maybe_unused]] const cplx *xa_other = sm.xa[1 - g];
+    // ring slot of block 2c + r: RING = 4 -> 2c + r; RING = 2 -> blocks 1, 2 at 0, 1
+    [[maybe_unused]] const cplx *k_own = &sm.ring[RING == 4 ? 2 * g + g : 0][0];
+    const cplx *k_oth = &sm.ring[RING == 4 ? 2 * g + (1 - g) : RING == 2 ? g : 0][0];
+    const cplx *bsk_own = bsk + (size_t)g * (2 * P22_M) + (size_t)g * P22_M + t;
+    [[maybe_unused]] const cplx *bsk_oth =
+        bsk + (size_t)g * (2 * P22_M) + (size_t)(1 - g) * P22_M;
+    uint32_t own[32];
+    p22v4_own_init(acc_g, t, own);
+    [[maybe_unused]] uint64_t ct_next = (!STAGE_A && n > 0) ? ct[0] : 0;
+    [[maybe_unused]] uint32_t a_next = (STAGE_A && n > 0) ? sm.a_hat[0] : 0;
     for (uint32_t i = 0; i < n; i++) {
       uint32_t a;
       if constexpr (STAGE_A) {

@@ -1,12 +1,13 @@
 // tools/micro/phase_clocks.cu -- where do the cycles of ONE CMUX step go?
-// Replays the blind-rotation loop of the shipped two-CTA N = 2048 instance
-// (pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1>, lane-pair layout: same phase
-// functions, same order, same barriers) with a clock64() read between phases,
+// Runs the blind-rotation loop of the shipped two-CTA N = 2048 instance
+// (pbs_n2048_k1_l1_v6_kernel<2, true, 2, 1>, lane-pair layout) -- the kernel's
+// own p22_lanepair_loop, with a probe that reads clock64() between phases --
 // for exchange 2 through the warp's own rows (x2m_*, X2 = 1, the shipped one)
-// and through half-warp shuffles (x2h_*, X2 = 0).  Every SM runs 1 or 2 CTAs;
-// the tool prints the average cycles per phase of warp 0 of CTA 0.  The clock
-// reads order the phases of a warp, so the sum is a little above the step time
-// of the kernel.  Measurement tool only (not part of the library).
+// and through half-warp shuffles (x2h_*, X2 = 0), on a synthetic accumulator
+// and mask.  Every SM runs 1 or 2 CTAs; the tool prints the average cycles per
+// phase of warp 0 of CTA 0.  The clock reads order the phases of a warp, so the
+// sum is a little above the step time of the kernel.  Measurement tool only
+// (not part of the library).
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I../../tfhe-rs_b200/csrc -o phase_clocks phase_clocks.cu
 //   ./phase_clocks <CTAs per SM: 1 or 2>
 #include <cstdio>
@@ -22,6 +23,19 @@ __device__ __forceinline__ long long clk() {
   return c;
 }
 
+// cycles per phase, summed over the steps: 32-bit sums (918 steps of a few
+// thousand cycles) keep the loop free of spills
+struct ClockProbe {
+  uint32_t acc[NPH] = {};
+  long long t0;
+  __device__ __forceinline__ void begin() { t0 = clk(); }
+  __device__ __forceinline__ void lap(int p) {
+    const long long t1 = clk();
+    acc[p] += (uint32_t)(t1 - t0);
+    t0 = t1;
+  }
+};
+
 template <int X2>
 __global__ void __launch_bounds__(128, 2)
 timed_lanepair(const cplx *__restrict__ bsk, const Fft1024Tables *__restrict__ tables,
@@ -30,7 +44,7 @@ timed_lanepair(const cplx *__restrict__ bsk, const Fft1024Tables *__restrict__ t
   using Smem = P22SmemV6<2, true>;
   Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
   const int tid = threadIdx.x;
-  const int g = (tid >> 4) & 1, t = ((tid >> 5) << 4) | (tid & 15);
+  const int t = p22lp_t(tid);
   if (tid == 0) { mbar_init(&sm.bar, 1); mbar_fence_init(); }
   for (uint32_t i = tid; i < n + 8; i += 128)
     sm.a_hat[i] = (uint16_t)(1 + ((i * 2654435761u + blockIdx.x * 40503u) % 4095u));
@@ -42,58 +56,12 @@ timed_lanepair(const cplx *__restrict__ bsk, const Fft1024Tables *__restrict__ t
 #pragma unroll
   for (int e = 0; e < 15; e++) tw3[e] = tables->pass3[t][e];
   __syncthreads();
-  auto tma_issue = [&](uint32_t i) {
-    mbar_arrive_expect_tx(&sm.bar, 2u * P22_M * (uint32_t)sizeof(cplx));
-    tma_bulk_g2s(&sm.ring[0][0], bsk + (size_t)i * (4 * P22_M) + P22_M,
-                 2u * P22_M * (uint32_t)sizeof(cplx), &sm.bar);
-  };
-  if (tid == 0) tma_issue(0);
+  if (tid == 0) p22_ring_issue(&sm.ring[0][0], &sm.bar, bsk, 0);
   __syncthreads();
-  uint32_t *acc_g = sm.acc[g];
-  cplx *xa_g = sm.xa[g];
-  cplx *x2_rows = xa_g + 256 * (tid >> 5);
-  const cplx *k_oth = &sm.ring[g][0];
-  const cplx *bsk_own = bsk + (size_t)g * (2 * P22_M) + (size_t)g * P22_M + t;
-  uint32_t own[32];
-  p22v4_own_init(acc_g, t, own);
-  uint32_t acc[NPH]; // 32-bit sums (918 steps of a few thousand cycles) keep the replay free of spills
-  for (int p = 0; p < NPH; p++) acc[p] = 0;
-  long long t0, t1;
-#define LAP(p) t1 = clk(); acc[p] += (uint32_t)(t1 - t0); t0 = t1;
-  uint32_t a_next = sm.a_hat[0];
-  for (uint32_t i = 0; i < n; i++) {
-    const uint32_t a = a_next;
-    a_next = sm.a_hat[i + 1];
-    cplx v[16];
-    t0 = clk();
-    p22v4_load_digits<2>(acc_g, t, a, base_log, own, v);        LAP(0)
-    radix16_fwd(v, c_fft1024_pass1);                            LAP(1)
-    x1h_store_p1(xa_g, t, v); __syncthreads(); x1h_load_p2(xa_g, t, v); LAP(2)
-    pass2_fwd(v, tw2);                                          LAP(3)
-    if constexpr (X2 == 1) x2m_fwd(x2_rows, v); else x2h_fwd(v); LAP(4)
-    radix16_fwd(v, tw3);                                        LAP(5)
-    const size_t step = (size_t)i * (4 * P22_M);
-    cplx b_own[16];
-#pragma unroll
-    for (int b = 0; b < 16; b++) b_own[b] = ldcg_cplx(bsk_own + step + b * 64);
-    mbar_wait_parity(&sm.bar, i & 1u);                          LAP(6)
-#pragma unroll
-    for (int b = 0; b < 16; b++) {
-      const cplx o = shfl_xor_cplx(v[b], 16);
-      v[b] = cfma(o, k_oth[b * 64 + t], cmul(v[b], b_own[b]));
-    }
-    LAP(7)
-    radix16_inv(v, tw3);                                        LAP(8)
-    if constexpr (X2 == 1) x2m_inv(x2_rows, v); else x2h_inv(v); LAP(9)
-    pass2_inv(v, tw2);                                          LAP(10)
-    __syncwarp(); x1h_store_p2(xa_g, t, v); __syncthreads();
-    if (tid == 0 && i + 1 < n) tma_issue(i + 1);
-    x1h_load_p1(xa_g, t, v);                                    LAP(11)
-    radix16_inv(v, c_fft1024_pass1);                            LAP(12)
-    p22v4_acc_update(acc_g, t, v, own); __syncthreads();        LAP(13)
-  }
+  ClockProbe probe;
+  p22_lanepair_loop<X2>(sm, bsk, n, base_log, tw2, tw3, probe);
   if (tid == 0 && blockIdx.x == 0)
-    for (int p = 0; p < NPH; p++) out[p] = (unsigned long long)acc[p];
+    for (int p = 0; p < NPH; p++) out[p] = (unsigned long long)probe.acc[p];
   if (sm.acc[0][tid] == 0x12345678u) out[NPH] = 1; // keep results live
 }
 
