@@ -28,14 +28,14 @@ using namespace b200;
 
 namespace {
 
+// filled once, thread-safely: the replay is called from several threads at once
 const Fft1024Tables *tables() {
-  static Fft1024Tables tb;
-  static bool init = false;
-  if (!init) {
-    b200_fill_fft1024_tables(&tb);
-    init = true;
-  }
-  return &tb;
+  static const Fft1024Tables *tb = [] {
+    Fft1024Tables *t = new Fft1024Tables;
+    b200_fill_fft1024_tables(t);
+    return t;
+  }();
+  return tb;
 }
 
 uint64_t splitmix(uint64_t &s) {

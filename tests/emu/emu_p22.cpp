@@ -16,14 +16,17 @@
 #include "../../tfhe-rs_b200/csrc/pbs_n8192_phases.cuh"
 #include "../../tfhe-rs_b200/csrc/x2_shfl.cuh"
 
-static Fft1024Tables g_tables;
-static bool g_init = false;
+// The tables are filled on first use by whichever thread gets there first: the
+// replays are called from several threads at once (tests/
+// test_gpu_replay_words.py), and a function-local static is initialised exactly
+// once, before any thread sees it.
 static const Fft1024Tables *tables() {
-  if (!g_init) {
-    b200_fill_fft1024_tables(&g_tables);
-    g_init = true;
-  }
-  return &g_tables;
+  static const Fft1024Tables *tb = [] {
+    Fft1024Tables *t = new Fft1024Tables;
+    b200_fill_fft1024_tables(t);
+    return t;
+  }();
+  return tb;
 }
 
 struct Regs {
@@ -133,14 +136,13 @@ static void inv1024_shfl(const cplx *in_pos, cplx *out) {
 }
 
 // M = 256 (N = 512) transform of the pbs_n512 kernel: 16 emulated threads
-static Fft256Tables g_tables256;
-static bool g_init256 = false;
 static const Fft256Tables *tables256() {
-  if (!g_init256) {
-    b200_fill_fft256_tables(&g_tables256);
-    g_init256 = true;
-  }
-  return &g_tables256;
+  static const Fft256Tables *tb = [] {
+    Fft256Tables *t = new Fft256Tables;
+    b200_fill_fft256_tables(t);
+    return t;
+  }();
+  return tb;
 }
 static void fwd256(const cplx *in, cplx *out_pos) {
   const Fft256Tables *tb = tables256();
@@ -178,13 +180,13 @@ static void inv256(const cplx *in_pos, cplx *out) {
 }
 
 // M = 4096 (N = 8192) transform of the pbs_n8192 kernel: 256 emulated threads
-static Fft4096Tables *g_tables4096 = nullptr;
 static const Fft4096Tables *tables4096() {
-  if (!g_tables4096) {
-    g_tables4096 = new Fft4096Tables;
-    b200_fill_fft4096_tables(g_tables4096);
-  }
-  return g_tables4096;
+  static const Fft4096Tables *tb = [] {
+    Fft4096Tables *t = new Fft4096Tables;
+    b200_fill_fft4096_tables(t);
+    return t;
+  }();
+  return tb;
 }
 static void fwd4096(const cplx *in, cplx *out_pos) {
   const Fft4096Tables *tb = tables4096();
@@ -524,7 +526,11 @@ extern "C" void emu_bsk_convert_mb(const uint64_t *src, uint32_t n, uint32_t l,
 }
 
 
-template <int GROUPING>
+// LL = false: mirrors pbs_multibit_n2048_k1_kernel (bundle folded into the
+// MAC, mb_mac_step); LL = true: the low-latency mode, mb_bundle_kernel's bundle
+// of each step (mb_bundle_entry) then pbs_multibit_seq_kernel's MAC, 2 l terms
+// per slot summed from zero in (level, row) order
+template <int GROUPING, bool LL = false>
 static void emu_pbs_mb_impl(const cplx *bsk, const uint64_t *lut,
                             const uint64_t *ct, uint32_t n, uint32_t base_log,
                             uint32_t l, uint32_t num_many_lut,
@@ -587,6 +593,43 @@ static void emu_pbs_mb_impl(const cplx *bsk, const uint64_t *lut,
         spec_store(sp.data() + (size_t)(lvl * 2 + g) * P22_M, t, v);
       END_THREADS
     }
+    if (LL) {
+      // the bundle of this step, [lvl][c][r][b * 64 + t]
+      std::vector<cplx> bun((size_t)l * 4 * P22_M);
+      for (uint32_t c = 0; c < 2; c++)
+        for (uint32_t b = 0; b < 16; b++)
+          for (int t = 0; t < 64; t++) {
+            const cplx *rows = bsk + mb_key_row(grp, c, b, 0, 0, 0, l, nggsw) + t;
+            auto key = [&](uint32_t sigma, int lvl, int r) {
+              return rows[((size_t)(lvl * 2 + r) * nggsw + sigma) * 64];
+            };
+            auto mono_row = [&](uint32_t deg) { return root[mb_base_exponent(deg, t)]; };
+            auto put = [&](auto &acc) {
+              for (uint32_t lvl = 0; lvl < l; lvl++)
+                for (int r = 0; r < 2; r++)
+                  bun[((lvl * 2 + c) * 2 + r) * P22_M + b * 64 + t] = acc[lvl][r];
+            };
+            if (l == 1) {
+              cplx acc[1][2];
+              mb_bundle_entry<(int)nggsw, 1>(key, mono_row, zeta, degs, mb_bitrev4(b), acc);
+              put(acc);
+            } else {
+              cplx acc[2][2];
+              mb_bundle_entry<(int)nggsw, 2>(key, mono_row, zeta, degs, mb_bitrev4(b), acc);
+              put(acc);
+            }
+          }
+      MB_THREADS
+        for (int b = 0; b < 16; b++) {
+          cplx out = cmake(0.0, 0.0);
+          for (uint32_t lvl = 0; lvl < l; lvl++)
+            for (int r = 0; r < 2; r++)
+              out = cfma(sp[((size_t)(lvl * 2 + r) * 16 + b) * 64 + t],
+                         bun[((lvl * 2 + g) * 2 + r) * P22_M + b * 64 + t], out);
+          v[b] = out;
+        }
+      END_THREADS
+    } else {
     MB_THREADS
       cplx mono_base[nggsw - 1];
       for (uint32_t s = 1; s < nggsw; s++)
@@ -604,6 +647,7 @@ static void emu_pbs_mb_impl(const cplx *bsk, const uint64_t *lut,
       for (int b = 0; b < 16; b++)
         v[b] = xa_g[b * 64 + t];
     END_THREADS
+    }
     MB_THREADS
       radix16_inv(v, tb->pass3[t]);
       x2_store_p3(xa_g, t, v);
@@ -631,6 +675,20 @@ static void emu_pbs_mb_impl(const cplx *bsk, const uint64_t *lut,
   }
   sample_extract_many_lut(out_base, 0, count, num_many_lut, lut_stride, acc.data(), P22_N,
                           1, P22_N, 0, 1, Torus32To64());
+}
+
+// mirrors the low-latency multi-bit mode (mb_bundle_kernel + pbs_multibit_seq_kernel)
+extern "C" void emu_pbs_mb_ll(const double *bsk_, const uint64_t *lut, const uint64_t *ct,
+                   uint32_t n, uint32_t base_log, uint32_t l, uint32_t grouping,
+                   uint32_t num_many_lut, uint32_t lut_stride, uint32_t count,
+                   uint64_t *out_base) {
+  const cplx *bsk = reinterpret_cast<const cplx *>(bsk_);
+  if (grouping == 2)
+    emu_pbs_mb_impl<2, true>(bsk, lut, ct, n, base_log, l, num_many_lut, lut_stride, count, out_base);
+  else if (grouping == 3)
+    emu_pbs_mb_impl<3, true>(bsk, lut, ct, n, base_log, l, num_many_lut, lut_stride, count, out_base);
+  else
+    emu_pbs_mb_impl<4, true>(bsk, lut, ct, n, base_log, l, num_many_lut, lut_stride, count, out_base);
 }
 
 extern "C" void emu_pbs_mb(const double *bsk_, const uint64_t *lut, const uint64_t *ct,

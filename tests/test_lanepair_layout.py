@@ -11,13 +11,10 @@ address patterns are bank-conflict free.  GPU: the instance is word-identical
 to the two-CTA instance of the other layout (variant 17, `n2048_v6<2,true,2>`)
 on the same keys and inputs."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 LANE_PAIR, OTHER_LAYOUT = "n2048_v6<2,true,2,1>", "n2048_v6<2,true,2>"
 
 
@@ -27,15 +24,10 @@ def emus(tmp_path_factory):
     floating-point contraction: the host compiler would otherwise fuse
     multiplies and adds differently in the two files, and word identity is a
     question of which operations run in which order."""
-    d = tmp_path_factory.mktemp("emu_lanepair")
-    gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-    libs = []
-    for src in ("emu_p22.cpp", "emu_lanepair.cpp"):
-        out = str(d / src.replace(".cpp", ".so"))
-        subprocess.check_call([gxx, "-O2", "-mavx2", "-mfma", "-ffp-contract=off", "-std=c++17", "-fPIC", "-shared",
-                               "-w", "-x", "c++", os.path.join(HERE, "emu", src), "-o", out])
-        libs.append(C.CDLL(out))
-    return libs
+    from tests.emu.build_emu import build_no_contract
+
+    libs = build_no_contract(str(tmp_path_factory.mktemp("emu_lanepair")))
+    return [C.CDLL(libs["emu_p22.cpp"]), C.CDLL(libs["emu_lanepair.cpp"])]
 
 
 @pytest.fixture(scope="module")

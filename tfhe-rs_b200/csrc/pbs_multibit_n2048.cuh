@@ -149,24 +149,15 @@ mb_bundle_kernel(cplx *__restrict__ bundle, const cplx *__restrict__ bsk,
     const uint32_t cnt = min((uint32_t)S, num_samples - s0);
     for (uint32_t ss = 0; ss < cnt; ss++) {
       cplx acc[L][2];
-#pragma unroll
-      for (int lvl = 0; lvl < L; lvl++)
-#pragma unroll
-        for (int r = 0; r < 2; r++)
-          acc[lvl][r] = KEY_IN_REGS ? kreg[0][lvl][r] : key(0, lvl, r);
-#pragma unroll
-      for (uint32_t sigma = 1; sigma < nggsw; sigma++) {
-        const uint32_t deg = degs[ss][sigma];
-        const cplx mono =
-            cmul(mono_tab[(size_t)deg * 64 + t], zeta[(deg * rb) & 15u]);
-#pragma unroll
-        for (int lvl = 0; lvl < L; lvl++)
-#pragma unroll
-          for (int r = 0; r < 2; r++)
-            acc[lvl][r] = cfma(KEY_IN_REGS ? kreg[sigma][lvl][r]
-                                           : key(sigma, lvl, r),
-                               mono, acc[lvl][r]);
-      }
+      mb_bundle_entry<nggsw, L>(
+          [&](uint32_t sigma, int lvl, int r) {
+            if constexpr (KEY_IN_REGS)
+              return kreg[sigma][lvl][r];
+            else
+              return key(sigma, lvl, r);
+          },
+          [&](uint32_t deg) { return mono_tab[(size_t)deg * 64 + t]; }, zeta,
+          degs[ss], rb, acc);
 #pragma unroll
       for (int lvl = 0; lvl < L; lvl++)
 #pragma unroll

@@ -203,6 +203,33 @@ B200_HD void mb_mac_step(const cplx *sp, const cplx *mono_base, const cplx *zeta
   }
 }
 
+// One entry of the low-latency mode's bundle (mb_bundle_kernel): at spectrum
+// slot (b, t) of one (group, column), for every level and row,
+//   bundle = B_0 + sum_{s >= 1} B_s * rho^{deg_s}
+// summed GGSW by GGSW from s = 1, the monomial as in mb_mac_step.  key(s, lvl,
+// r) gives the key value, mono_row(deg) = tau^{deg * (1 + 4*bitrev6(t))}, rb =
+// bitrev4(b).
+template <int NGGSW, int L, typename Key, typename MonoRow>
+B200_HD void mb_bundle_entry(Key key, MonoRow mono_row, const cplx *zeta,
+                             const uint32_t *degs, uint32_t rb,
+                             cplx acc[L][2]) {
+#pragma unroll
+  for (int lvl = 0; lvl < L; lvl++)
+#pragma unroll
+    for (int r = 0; r < 2; r++)
+      acc[lvl][r] = key(0u, lvl, r);
+#pragma unroll
+  for (uint32_t sigma = 1; sigma < (uint32_t)NGGSW; sigma++) {
+    const uint32_t deg = degs[sigma];
+    const cplx mono = cmul(mono_row(deg), zeta[(deg * rb) & 15u]);
+#pragma unroll
+    for (int lvl = 0; lvl < L; lvl++)
+#pragma unroll
+      for (int r = 0; r < 2; r++)
+        acc[lvl][r] = cfma(key(sigma, lvl, r), mono, acc[lvl][r]);
+  }
+}
+
 B200_HD void mb_acc_assign(uint32_t acc_lo[16], uint32_t acc_hi[16],
                            const cplx v[16]) {
 #pragma unroll

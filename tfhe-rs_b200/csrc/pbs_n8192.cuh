@@ -527,8 +527,13 @@ pbs_n8192_k1_l2_v2_kernel(uint64_t *__restrict__ lwe_out,
                                          : cfma(f[4 * q4 + bq], kv, out[4 * q4 + bq]);
             }
             if (ALL_ARRIVE) {
-              mbar_arrive(&sm.empty[c_slot]);
+              // the loads above are still in flight when a bare arrive issues
+              mbar_arrive_after_reads(&sm.empty[c_slot]);
             } else {
+              // no fence: in the compiled kernel lane 0's arrive issues after
+              // the warp's DMULs that wait on these loads, so they are done.
+              // That is the schedule, not a guarantee of the source;
+              // tests/test_gpu_replay_words.py would see a late read.
               __syncwarp();
               if ((t & 31) == 0)
                 mbar_arrive(&sm.empty[c_slot]);

@@ -43,6 +43,15 @@ __device__ __forceinline__ void mbar_arrive(unsigned long long *bar) {
                    smem_addr_u32(bar))
                : "memory");
 }
+// consumer release of a ring slot that this thread has read with plain loads,
+// arriving on the slot's barrier itself: the next async-proxy (TMA) write into
+// the slot must not overtake those reads.  The proxy fence makes the thread's
+// shared-memory reads complete first (MEMBAR.CTA + FENCE.VIEW.ASYNC.S); a bare
+// arrive may issue while the loads are still in flight.
+__device__ __forceinline__ void mbar_arrive_after_reads(unsigned long long *bar) {
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  mbar_arrive(bar);
+}
 __device__ __forceinline__ void mbar_wait_parity(unsigned long long *bar,
                                                  uint32_t parity) {
   asm volatile("{\n\t"
