@@ -198,6 +198,27 @@ class CudaBitCircuitRunner:
         out.record_stream(caller)
         return out
 
+    def run_schedule(self, key, sched: bc.Schedule, instance) -> torch.Tensor:
+        """A schedule laid out as tables rather than compiled from a circuit
+        (`radix_find`'s cross-candidate trees: one instance, inputs at pool
+        rows 0 ..), in one call; `key` (hashable) names its device tables.
+        instance: [num_instance_inputs, big + 1].  Returns the outputs, with
+        the stream rules of `run`."""
+        st = self.streams.streams[0]
+        out = self._run_chunk(key, sched, None, instance, None)
+        caller = torch.cuda.current_stream(self.device)
+        caller.wait_stream(st)
+        out.record_stream(caller)
+        return out
+
+    def trivial(self, digits) -> torch.Tensor:
+        """noiseless blocks of the given messages (mask 0, body m * delta),
+        [len(digits), big + 1] on the caller's current stream"""
+        big = self.skey.big_dim
+        out = torch.zeros((len(digits), big + 1), dtype=torch.int64, device=self.device)
+        out[:, big] = torch.tensor([int(d) * DELTA for d in digits], dtype=torch.int64)
+        return out
+
     def _run_chunk(self, circuit: bc.Circuit, sched: bc.Schedule, shared, instance, iconsts) -> torch.Tensor:
         L = _lib.lib()
         skey, bsk, ksk = self.skey, self.skey.bsk, self.skey.ksk

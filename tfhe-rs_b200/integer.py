@@ -323,7 +323,8 @@ class CudaRadixServerKey:
     (integer/gpu/server_key/radix/mul.rs:167), and comparisons, selects,
     additions, subtractions, bitwise operations, their clear-operand forms,
     signed overflow flags, abs, erc7984's transfer (`radix`), products and
-    sums (`radix_mul`), divisions (`radix_div`) and shifts, rotations and bit counts (`radix_bits`), compiled to KS -> PBS
+    sums (`radix_mul`), divisions (`radix_div`), shifts, rotations and bit counts (`radix_bits`), and vector find
+    and the key-value store's encrypted-key operations (`radix_find`), compiled to KS -> PBS
     layers and run by a bit-circuit runner of its own (created on first use) with `b200_bit_circuit_64_async`.
 
     Those operations take ciphertexts of one kind (unsigned or signed), one
@@ -820,3 +821,125 @@ class CudaRadixServerKey:
         """(`ilog2`, ct > 0): the flag compares with ct's own signedness, as
         tfhe-rs does, so it is 0 for a negative signed ct"""
         return self._count("checked_ilog2", ct)
+
+    # -- vector find and the key-value store (`radix_find`, `kv_store`) ---------
+    # Lists are Python sequences of ciphertexts holding one integer each, of
+    # one kind and block count; indexes are unsigned.  Empty lists and stores
+    # give tfhe-rs' trivial results.
+    def match_value(self, ct, matches):
+        """(the output of the (input, output) pair of `matches` whose input
+        equals the unsigned ct, else 0, on enough blocks for the largest
+        output; [a match was found]).  Inputs must be unique and fit ct."""
+        from . import radix_find
+
+        return radix_find.match_value(self, ct, matches)
+
+    def match_value_or(self, ct, matches, or_value):
+        """the output of the matching pair, or the clear `or_value` when none
+        matches, on enough blocks for both"""
+        from . import radix_find
+
+        return radix_find.match_value_or(self, ct, matches, or_value)
+
+    def contains(self, cts, value):
+        """[the encrypted value equals an entry of cts]"""
+        from . import radix_find
+
+        return radix_find.contains(self, cts, value)
+
+    def contains_clear(self, cts, clear):
+        """[the clear value equals an entry of cts]"""
+        from . import radix_find
+
+        return radix_find.contains_clear(self, cts, clear)
+
+    def is_in_clears(self, ct, clears):
+        """[ct equals one of the clears]"""
+        from . import radix_find
+
+        return radix_find.is_in_clears(self, ct, clears)
+
+    def index_in_clears(self, ct, clears):
+        """(index of ct in clears, found) on enough blocks for len - 1; 0 when
+        not found"""
+        from . import radix_find
+
+        return radix_find.index_in_clears(self, ct, clears)
+
+    def first_index_in_clears(self, ct, clears):
+        """(index of the first occurrence of ct in clears, found)"""
+        from . import radix_find
+
+        return radix_find.index_in_clears(self, ct, clears, first=True)
+
+    def index_of(self, cts, value):
+        """(index of the encrypted value in cts, found)"""
+        from . import radix_find
+
+        return radix_find.index_of(self, cts, value=value)
+
+    def index_of_clear(self, cts, clear):
+        """(index of the clear value in cts, found)"""
+        from . import radix_find
+
+        return radix_find.index_of(self, cts, clear=clear)
+
+    def first_index_of(self, cts, value):
+        """(index of the first entry of cts equal to the encrypted value, found)"""
+        from . import radix_find
+
+        return radix_find.index_of(self, cts, value=value, first=True)
+
+    def first_index_of_clear(self, cts, clear):
+        """(index of the first entry of cts equal to the clear value, found)"""
+        from . import radix_find
+
+        return radix_find.index_of(self, cts, clear=clear, first=True)
+
+    def all_eq_slices(self, lhs, rhs):
+        """[lhs and rhs have one length and equal entries pairwise]"""
+        from . import radix_find
+
+        return radix_find.all_eq_slices(self, lhs, rhs)
+
+    def contains_sub_slice(self, lhs, pattern):
+        """[the non-empty pattern occurs in lhs as a contiguous run]"""
+        from . import radix_find
+
+        return radix_find.contains_sub_slice(self, lhs, pattern)
+
+    def kv_store_get(self, store, key):
+        """(the value of `store` (a kv_store.CudaKVStore) under the key equal
+        to the encrypted `key`, else 0; found)"""
+        from . import radix_find
+
+        return radix_find.kv_store_get(self, store, key)
+
+    def kv_store_update(self, store, key, new_value):
+        """store[key] = new_value for the encrypted key, every entry rewritten
+        as sel_i ? new_value : v_i in one call; returns found"""
+        from . import radix_find
+
+        return radix_find.kv_store_update(self, store, key, new_value)
+
+    def kv_store_map(self, store, key, func):
+        """(old, new, found): old = store[key], new = func(old) (any callable
+        on a ciphertext, for example a method of this key), store[key] = new"""
+        from . import radix_find
+
+        return radix_find.kv_store_map(self, store, key, func)
+
+    def kv_store_contains_key(self, store, key):
+        from . import radix_find
+
+        return radix_find.kv_store_contains_key(self, store, key)
+
+    def kv_store_contains_value(self, store, value):
+        from . import radix_find
+
+        return radix_find.kv_store_contains_value(self, store, value)
+
+    def kv_store_contains_clear_value(self, store, clear):
+        from . import radix_find
+
+        return radix_find.kv_store_contains_clear_value(self, store, clear)
