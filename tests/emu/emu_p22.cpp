@@ -14,6 +14,7 @@
 #include "../../tfhe-rs_b200/csrc/pbs_multibit_n2048_phases.cuh"
 #include "../../tfhe-rs_b200/csrc/pbs_generic_phases.cuh"
 #include "../../tfhe-rs_b200/csrc/pbs_n8192_phases.cuh"
+#include "../../tfhe-rs_b200/csrc/pbs_n512_phases.cuh"
 #include "../../tfhe-rs_b200/csrc/x2_shfl.cuh"
 
 // The tables are filled on first use by whichever thread gets there first: the
@@ -825,4 +826,291 @@ extern "C" void emu_digits_u32_reference_ties(uint32_t x, uint32_t base_log, uin
   digits_u32<2>(x, base_log, l, d, false);
   out[0] = d[0];
   out[1] = d[1];
+}
+
+// ---------------------------------------------------------------------------
+// any-(N, k, l) kernel (pbs_generic.cuh), classic and multi-bit, 64- or 32-bit
+// torus: one CTA of 256 threads replayed phase by phase with the kernel's own
+// phases (modulus switch, rotation, gen_decompose, radix-2 levels, gen_mac,
+// gen_acc_update, sample extraction with TorusIo's widen / narrow).  Both
+// variants of the kernel (shared memory and global workspace) compute the same
+// words: they differ only in where the working set lives.
+// ---------------------------------------------------------------------------
+namespace {
+constexpr uint32_t GEN_THREADS = 256, GEN_MAX_LOGM = 13; // N = 16384
+
+// twiddle and root tables of every transform size, filled once, as the
+// backend's device tables are (b200_fill_generic_tables)
+struct GenTables {
+  std::vector<cplx> tw, root;
+};
+const GenTables &gen_tables(uint32_t logM) {
+  static const std::vector<GenTables> *all = [] {
+    auto *v = new std::vector<GenTables>(GEN_MAX_LOGM + 1);
+    for (uint32_t L = 1; L <= GEN_MAX_LOGM; L++) {
+      (*v)[L].tw.resize(1u << L);
+      (*v)[L].root.resize(4u << L);
+      b200_fill_generic_tables(L, (*v)[L].tw.data(), (*v)[L].root.data());
+    }
+    return v;
+  }();
+  return (*all)[logM];
+}
+
+uint32_t log2_exact(uint32_t x) {
+  uint32_t r = 0;
+  while ((1u << r) < x)
+    r++;
+  return r;
+}
+
+// mirrors bsk_convert_generic_kernel over `polys` polynomials of N words
+template <typename Torus>
+void emu_bsk_convert_generic_impl(const Torus *src, size_t polys, uint32_t N, cplx *dst) {
+  const uint32_t M = N >> 1, logM = log2_exact(M);
+  const GenTables &tb = gen_tables(logM);
+  const double scale = ldexp(1.0, -64 - (int)logM);
+  std::vector<cplx> buf(M);
+  for (size_t b = 0; b < polys; b++) {
+    const Torus *p = src + b * N;
+    for (uint32_t j = 0; j < M; j++)
+      buf[j] = cmake(ll_to_double((int64_t)TorusIo<Torus>::widen(p[j])) * scale,
+                     ll_to_double((int64_t)TorusIo<Torus>::widen(p[j + M])) * scale);
+    for (uint32_t L = 1; L <= logM; L++)
+      for (uint32_t tid = 0; tid < 256; tid++)
+        gen_fwd_level(buf.data(), logM, L, tb.tw.data(), 1, tid, 256);
+    std::memcpy(dst + b * M, buf.data(), M * sizeof(cplx));
+  }
+}
+
+// mirrors pbs_generic_kernel for one sample (out_idx 0 of a batch of `count`)
+template <typename Torus>
+void emu_pbs_generic_impl(const cplx *bsk, const Torus *lut, const Torus *ct, uint32_t n, uint32_t k, uint32_t N,
+                          uint32_t base_log, uint32_t l, uint32_t grouping, int centered_ms, int ties_even,
+                          uint32_t num_many_lut, uint32_t lut_stride, uint32_t count, Torus *out_base) {
+  using Io = TorusIo<Torus>;
+  constexpr uint32_t NT = GEN_THREADS;
+  const uint32_t M = N >> 1, logM = log2_exact(M), log_mod = logM + 2;
+  const GenTables &tb = gen_tables(logM);
+  const bool multibit = grouping > 1;
+  std::vector<uint64_t> acc((size_t)(k + 1) * N);
+  std::vector<cplx> F((size_t)l * (k + 1) * M), out((size_t)(k + 1) * M);
+  std::vector<uint32_t> a_hat(n + 1);
+  uint32_t degs[16] = {0};
+  CenteredMsSums sums;
+  if (!multibit)
+    for (uint32_t i = 0; i < n; i++) {
+      const uint64_t a = Io::widen(ct[i]);
+      a_hat[i] = modulus_switch_u64(a, log_mod);
+      if (centered_ms)
+        sums.add(a, log_mod);
+    }
+  const uint32_t b_hat = ms_b_hat(Io::widen(ct[n]), !multibit && centered_ms, &sums.half, &sums.dbl, 1, log_mod);
+  rotate_lut(acc.data(), N, lut, k + 1, N, b_hat, 0, 1, [](Torus x) { return Io::widen(x); });
+  const uint32_t nggsw = multibit ? (1u << grouping) : 1u;
+  const uint32_t steps = multibit ? n / grouping : n;
+  const size_t ggsw_len = (size_t)l * (k + 1) * (k + 1) * M;
+  for (uint32_t i = 0; i < steps; i++) {
+    uint32_t a = 0;
+    if (multibit) {
+      for (uint32_t s = 0; s < nggsw; s++) {
+        uint64_t sum = 0;
+        for (uint32_t u = 0; u < grouping; u++)
+          if ((s >> (grouping - 1 - u)) & 1u)
+            sum += Io::widen(ct[i * grouping + u]);
+        degs[s] = modulus_switch_u64(sum, log_mod);
+      }
+    } else {
+      a = a_hat[i];
+      if (a == 0)
+        continue;
+    }
+    for (uint32_t tid = 0; tid < NT; tid++)
+      gen_decompose(acc.data(), F.data(), N, k, base_log, l, a, multibit, tid, NT, ties_even != 0);
+    for (uint32_t L = 1; L <= logM; L++)
+      for (uint32_t tid = 0; tid < NT; tid++)
+        gen_fwd_level(F.data(), logM, L, tb.tw.data(), l * (k + 1), tid, NT);
+    for (uint32_t tid = 0; tid < NT; tid++)
+      gen_mac(F.data(), out.data(), bsk + (size_t)i * nggsw * ggsw_len, N, k, l, nggsw, degs, tb.root.data(), tid,
+              NT, HostLoader());
+    for (uint32_t L = logM; L >= 1; L--)
+      for (uint32_t tid = 0; tid < NT; tid++)
+        gen_inv_level(out.data(), logM, L, tb.tw.data(), k + 1, tid, NT);
+    for (uint32_t tid = 0; tid < NT; tid++)
+      gen_acc_update(acc.data(), out.data(), N, k, multibit, tid, NT);
+  }
+  sample_extract_many_lut(out_base, 0, count, num_many_lut, lut_stride, acc.data(), N, k, N, 0, 1,
+                          [](uint64_t x) { return Io::narrow(x); });
+}
+} // namespace
+
+// torus_bits 64: u64 words; 32: u32 words (the _32 entry points)
+extern "C" void emu_bsk_convert_generic(const void *src, uint64_t polys, uint32_t N, int torus_bits, double *dst) {
+  cplx *d = reinterpret_cast<cplx *>(dst);
+  if (torus_bits == 32)
+    emu_bsk_convert_generic_impl(static_cast<const uint32_t *>(src), polys, N, d);
+  else
+    emu_bsk_convert_generic_impl(static_cast<const uint64_t *>(src), polys, N, d);
+}
+
+extern "C" void emu_pbs_generic(const double *bsk_, const void *lut, const void *ct, uint32_t n, uint32_t k,
+                                uint32_t N, uint32_t base_log, uint32_t l, uint32_t grouping, int centered_ms,
+                                int ties_even, uint32_t num_many_lut, uint32_t lut_stride, uint32_t count,
+                                int torus_bits, void *out_base) {
+  const cplx *bsk = reinterpret_cast<const cplx *>(bsk_);
+  if (torus_bits == 32)
+    emu_pbs_generic_impl(bsk, static_cast<const uint32_t *>(lut), static_cast<const uint32_t *>(ct), n, k, N,
+                         base_log, l, grouping, centered_ms, ties_even, num_many_lut, lut_stride, count,
+                         static_cast<uint32_t *>(out_base));
+  else
+    emu_pbs_generic_impl(bsk, static_cast<const uint64_t *>(lut), static_cast<const uint64_t *>(ct), n, k, N,
+                         base_log, l, grouping, centered_ms, ties_even, num_many_lut, lut_stride, count,
+                         static_cast<uint64_t *>(out_base));
+}
+
+// ---------------------------------------------------------------------------
+// N = 512, l = 1, k <= 4 register kernel (pbs_n512.cuh): one LWE of the CTA,
+// 16 (k + 1) threads, replayed with the kernel's phases (pbs_n512_phases.cuh).
+// The G LWEs of a CTA and the spare thread groups of a partial last group do
+// not change an LWE's words; the key mode does (the two MACs sum the rows in
+// different orders).
+// ---------------------------------------------------------------------------
+// mirrors bsk_convert_n512_kernel for polynomials first .. first + count - 1 of
+// the key: src [i][r][c][N] (l = 1), dst [i][c][r][b][q]
+extern "C" void emu_bsk_convert_n512(const uint64_t *src, uint32_t k, uint64_t first, uint64_t count,
+                                     double *dst_) {
+  cplx *dst = reinterpret_cast<cplx *>(dst_);
+  const Fft256Tables *tb = tables256();
+  const uint64_t P = k + 1;
+  std::vector<Regs> R(16);
+  std::vector<cplx> xb(P512_M);
+  for (uint64_t poly = first; poly < first + count; poly++) {
+    const uint64_t c = poly % P, r = (poly / P) % P, i = poly / (P * P);
+    for (int u = 0; u < 16; u++) {
+      n512_key_load(src + poly * P512_N, u, R[u].v);
+      radix16_fwd(R[u].v, tb->pass1);
+      xq_store_p1(xb.data(), u, R[u].v);
+    }
+    for (int u = 0; u < 16; u++) {
+      xq_load_p2(xb.data(), u, R[u].v);
+      radix16_fwd(R[u].v, tb->pass2[u]);
+      spec256_store(dst + ((i * P + c) * P + r) * P512_M, u, R[u].v);
+    }
+  }
+}
+
+// Fourier MAC of the register mode (pbs_n512_kernel<K, 2, false>), restated
+// from the kernel's loop: the same sum from row 0 up, the key
+// (`krow`: the P rows of this thread's column, element u) streaming through a
+// ring of three 8-value chunks; the first two are requested before `barrier`
+// (the CTA barrier after which every spectrum of xs_l is stored)
+template <int P, typename Load, typename Barrier>
+static void n512_mac_regs(cplx v[16], const cplx *xs_l, const cplx *krow, int u,
+                           Load load, Barrier barrier) {
+  cplx kbuf[3][8];
+  auto key_chunk = [&](int ch, cplx (&dst)[8]) {
+    const int r = ch >> 1, hb = (ch & 1) * 8;
+#pragma unroll
+    for (int b = 0; b < 8; b++)
+      dst[b] = load(krow + (size_t)r * P512_M + (hb + b) * 16);
+  };
+  key_chunk(0, kbuf[0]);
+  key_chunk(1, kbuf[1]);
+  barrier();
+  // ---- Fourier MAC: out[b] = sum_r spec_r[b][q] * key[i][p][r][b][q] -------
+#pragma unroll
+  for (int ch = 0; ch < 2 * P; ch++) {
+    const int r = ch >> 1, hb = (ch & 1) * 8;
+    if (ch + 2 < 2 * P)
+      key_chunk(ch + 2, kbuf[(ch + 2) % 3]);
+#pragma unroll
+    for (int b = 0; b < 8; b++) {
+      const cplx f = xs_l[(size_t)r * P512_M + (hb + b) * 16 + u];
+      v[hb + b] = r == 0 ? cmul(f, kbuf[ch % 3][b]) : cfma(f, kbuf[ch % 3][b], v[hb + b]);
+    }
+  }
+}
+
+template <int P>
+static void emu_pbs_n512_impl(const cplx *bsk, const uint64_t *lut, const uint64_t *ct, uint32_t n,
+                              uint32_t base_log, int centered_ms, bool ring, uint32_t num_many_lut,
+                              uint32_t lut_stride, uint32_t count, uint64_t *out_base) {
+  const Fft256Tables *tb = tables256();
+  const uint32_t log_mod = 10;
+  std::vector<uint16_t> a_hat(n);
+  CenteredMsSums sums;
+  for (uint32_t i = 0; i < n; i++) {
+    a_hat[i] = (uint16_t)modulus_switch_u64(ct[i], log_mod);
+    if (centered_ms)
+      sums.add(ct[i], log_mod);
+  }
+  const uint32_t b_hat = ms_b_hat(ct[n], centered_ms, &sums.half, &sums.dbl, 1, log_mod);
+  std::vector<uint32_t> acc(P * P512_N);
+  for (uint32_t j = 0; j < (uint32_t)(P * P512_N); j++) {
+    const uint32_t r = j >> 9, jj = j & (P512_N - 1);
+    acc[r * P512_N + jj] = torus64_to_32(rot_div_coeff(lut + r * P512_N, P512_N, jj, b_hat));
+  }
+  std::vector<Regs> R(16 * P);
+  std::vector<cplx> xs(P * P512_M);
+#define N512_THREADS                                                           \
+  for (int tl = 0; tl < 16 * P; tl++) {                                        \
+    const int p = tl >> 4, u = tl & 15;                                        \
+    cplx *v = R[tl].v;                                                         \
+    uint32_t *acc_p = acc.data() + p * P512_N;                                 \
+    cplx *xs_p = xs.data() + p * P512_M;                                       \
+    (void)v; (void)acc_p; (void)xs_p;
+  N512_THREADS
+    for (int j1 = 0; j1 < 16; j1++) {
+      R[tl].own[j1] = acc_p[16 * j1 + u];
+      R[tl].own[16 + j1] = acc_p[16 * j1 + u + P512_M];
+    }
+  END_THREADS
+  const size_t key_step = (size_t)P * P * P512_M;
+  for (uint32_t i = 0; i < n; i++) { // every step, a = 0 included, as the kernel
+    const uint32_t a = a_hat[i];
+    N512_THREADS
+      n512_load_digits(acc_p, u, a, base_log, R[tl].own, v);
+      radix16_fwd(v, tb->pass1);
+      xq_store_p1(xs_p, u, v);
+    END_THREADS
+    N512_THREADS
+      xq_load_p2(xs_p, u, v);
+      radix16_fwd(v, tb->pass2[u]);
+    END_THREADS
+    N512_THREADS
+      spec256_store(xs_p, u, v);
+    END_THREADS
+    N512_THREADS
+      const cplx *block = bsk + (size_t)i * key_step + (size_t)p * (P * P512_M);
+      if (ring)
+        n512_mac_ring<P>(v, xs.data(), block, p, u, HostLoader());
+      else
+        n512_mac_regs<P>(v, xs.data(), block + u, u, HostLoader(), [] {});
+    END_THREADS
+    N512_THREADS
+      radix16_inv(v, tb->pass2[u]);
+      xq_store_p2(xs_p, u, v);
+    END_THREADS
+    N512_THREADS
+      xq_load_p1(xs_p, u, v);
+      radix16_inv(v, tb->pass1);
+      n512_acc_update(acc_p, u, v, R[tl].own);
+    END_THREADS
+  }
+  sample_extract_many_lut(out_base, 0, count, num_many_lut, lut_stride, acc.data(), P512_N, P - 1, P512_N, 0, 1,
+                          Torus32To64());
+}
+
+// ring != 0: the TMA key-ring instances (n512<k,G,true>); 0: the register
+// key-ring instances (n512<k,2,false>)
+extern "C" void emu_pbs_n512(const double *bsk_, const uint64_t *lut, const uint64_t *ct, uint32_t n, uint32_t k,
+                             uint32_t base_log, int centered_ms, int ring, uint32_t num_many_lut,
+                             uint32_t lut_stride, uint32_t count, uint64_t *out_base) {
+  const cplx *bsk = reinterpret_cast<const cplx *>(bsk_);
+  switch (k) {
+  case 1: return emu_pbs_n512_impl<2>(bsk, lut, ct, n, base_log, centered_ms, ring, num_many_lut, lut_stride, count, out_base);
+  case 2: return emu_pbs_n512_impl<3>(bsk, lut, ct, n, base_log, centered_ms, ring, num_many_lut, lut_stride, count, out_base);
+  case 3: return emu_pbs_n512_impl<4>(bsk, lut, ct, n, base_log, centered_ms, ring, num_many_lut, lut_stride, count, out_base);
+  default: return emu_pbs_n512_impl<5>(bsk, lut, ct, n, base_log, centered_ms, ring, num_many_lut, lut_stride, count, out_base);
+  }
 }

@@ -44,24 +44,6 @@ static inline size_t generic_smem_bytes(uint32_t n, uint32_t k, uint32_t N,
 // over the samples -- the role of the reference's "no shared memory" variants
 // (programmable_bootstrap_classic.cuh: get_buffer_size_full_sm_.. / partial_sm).
 //
-// Torus = uint64_t: the 64-bit ABI.  Torus = uint32_t: the u32 torus of
-// cuda_programmable_bootstrap_lwe_ciphertext_vector_32_async (ciphertexts,
-// accumulators AND index vectors are u32, programmable_bootstrap.h:72-79): words
-// are widened to the top half of a u64 on the way in and rounded back to 32
-// bits on the way out; the blind rotation itself is the same 64-bit path.
-template <typename Torus> struct TorusIo {
-  static constexpr uint32_t SHIFT = 64 - 8 * sizeof(Torus);
-  __device__ static __forceinline__ uint64_t widen(Torus x) {
-    return (uint64_t)x << SHIFT;
-  }
-  __device__ static __forceinline__ Torus narrow(uint64_t x) {
-    if constexpr (SHIFT == 0)
-      return (Torus)x;
-    else
-      return (Torus)((x + ((uint64_t)1 << (SHIFT - 1))) >> SHIFT);
-  }
-};
-
 template <int NTHREADS, bool GLOBAL_WS = false, typename Torus = uint64_t>
 __global__ void __launch_bounds__(NTHREADS)
 pbs_generic_kernel(Torus *__restrict__ lwe_out,

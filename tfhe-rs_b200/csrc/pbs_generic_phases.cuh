@@ -30,6 +30,24 @@ static inline void b200_fill_generic_tables(uint32_t logM, cplx *tw,
   }
 }
 
+// Torus = uint64_t: the 64-bit ABI.  Torus = uint32_t: the u32 torus of
+// cuda_programmable_bootstrap_lwe_ciphertext_vector_32_async (ciphertexts,
+// accumulators AND index vectors are u32, programmable_bootstrap.h:72-79): words
+// are widened to the top half of a u64 on the way in and rounded back to 32
+// bits on the way out; the blind rotation itself is the same 64-bit path.
+template <typename Torus> struct TorusIo {
+  static constexpr uint32_t SHIFT = 64 - 8 * sizeof(Torus);
+  B200_HD static uint64_t widen(Torus x) {
+    return (uint64_t)x << SHIFT;
+  }
+  B200_HD static Torus narrow(uint64_t x) {
+    if constexpr (SHIFT == 0)
+      return (Torus)x;
+    else
+      return (Torus)((x + ((uint64_t)1 << (SHIFT - 1))) >> SHIFT);
+  }
+};
+
 // one forward level L over `npolys` consecutive polynomials of M complex
 B200_HD void gen_fwd_level(cplx *buf, uint32_t logM, uint32_t L,
                            const cplx *tw, uint32_t npolys, uint32_t tid,

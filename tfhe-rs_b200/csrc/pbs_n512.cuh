@@ -25,13 +25,11 @@
 //     (c, q) reads 16 contiguous bytes per (r, b), a half-warp 256 contiguous.
 #pragma once
 #include "pbs_n2048.cuh" // ldcg_cplx, phases
+#include "pbs_n512_phases.cuh"
 
 #include <cuda_runtime.h>
 
 namespace b200 {
-
-#define P512_N 512
-#define P512_M 256
 
 __constant__ cplx c_fft256_pass1[15];
 
@@ -40,6 +38,11 @@ __device__ __forceinline__ cplx ldnc_cplx(const cplx *p) {
   const double2 v = __ldg(reinterpret_cast<const double2 *>(p));
   return cmake(v.x, v.y);
 }
+
+// key loader of the ring mode's MAC: the shared ring
+struct SmemLoader {
+  __device__ __forceinline__ cplx operator()(const cplx *p) const { return *p; }
+};
 
 // RING: the Fourier key block of a step ((k+1)^2 x 4 KiB, contiguous in the
 // layout below) is brought into shared memory by the TMA unit a whole step ahead
@@ -60,57 +63,6 @@ struct N512Smem {
   long long red_dbl[G][4];
   unsigned long long bar;
 };
-
-// rotate + decompose for N = 512 (p22v4_load_digits with stride 16): thread u
-// holds complex coefficients j = 16*j1 + u (re <- coefficient j, im <- j + 256)
-__device__ __forceinline__ void n512_load_digits(const uint32_t *acc_p, int u,
-                                                 uint32_t a, uint32_t base_log,
-                                                 const uint32_t own[32],
-                                                 cplx v[16]) {
-  const uint32_t d = a & (P512_N - 1);
-  const bool neg0 = (a >> 9) != 0u; // a >= N
-  const uint32_t half = 1u << (31 - base_log);
-  const uint32_t sh = 32 - base_log;
-  const int32_t tie_below = (int32_t)(0x80000000u + half);
-  const int32_t plus_half_base = (int32_t)(1u << (base_log - 1));
-  const uint32_t base4 = ((uint32_t)u - d) * 4u; // 4 * (j - d) for j1 = 0
-  const unsigned char *accb = reinterpret_cast<const unsigned char *>(acc_p);
-#pragma unroll
-  for (int j1 = 0; j1 < 16; j1++) {
-    const uint32_t ub0 = base4 + 64u * j1;       // 4 * (j - d)
-    const uint32_t ub1 = ub0 + 4u * P512_M;      // 4 * (j + M - d)
-    const uint32_t ib0 = ub0 & (4u * P512_N - 4u);
-    const uint32_t r0 = *reinterpret_cast<const uint32_t *>(accb + ib0);
-    const uint32_t r1 =
-        *reinterpret_cast<const uint32_t *>(accb + (ib0 ^ (4u * P512_M)));
-    const bool n0 = ((int32_t)ub0 < 0) != neg0;
-    const bool n1 = ((int32_t)ub1 < 0) != neg0;
-    const uint32_t x0 = n0 ? (0u - r0) - own[j1] : r0 - own[j1];
-    const uint32_t x1 = n1 ? (0u - r1) - own[16 + j1] : r1 - own[16 + j1];
-    int32_t d0 = (int32_t)(x0 + half) >> sh;
-    int32_t d1 = (int32_t)(x1 + half) >> sh;
-    // balanced tie (decomposer.rs:163-188): x in [2^31, 2^31 + half) -> +B/2
-    if ((int32_t)x0 < tie_below)
-      d0 = plus_half_base;
-    if ((int32_t)x1 < tie_below)
-      d1 = plus_half_base;
-    v[j1] = cmake(int_to_double(d0), int_to_double(d1));
-  }
-}
-
-__device__ __forceinline__ void n512_acc_update(uint32_t *acc_p, int u,
-                                                const cplx v[16],
-                                                uint32_t own[32]) {
-#pragma unroll
-  for (int j1 = 0; j1 < 16; j1++) {
-    const uint32_t j = 16u * j1 + (uint32_t)u;
-    // own[] is the current accumulator word: no read of shared memory
-    own[j1] += scaled_double_to_torus32(v[j1].re);
-    own[16 + j1] += scaled_double_to_torus32(v[j1].im);
-    acc_p[j] = own[j1];
-    acc_p[j + P512_M] = own[16 + j1];
-  }
-}
 
 // persistent grid (see below), block = 16 (K+1) G
 template <int K, int G, bool RING = false>
@@ -249,24 +201,7 @@ pbs_n512_kernel(uint64_t *__restrict__ lwe_out,
       // ---- Fourier MAC from shared memory ------------------------------------
       // the thread's own spectrum is still in registers: start with row r = p,
       // then walk the other rows cyclically (16 fewer 128-bit loads per thread)
-      const cplx *kcol = &sm.ring[p * P][0];
-      {
-        const cplx *kp = kcol + (size_t)p * P512_M + u;
-#pragma unroll
-        for (int b = 0; b < 16; b++)
-          v[b] = cmul(v[b], kp[b * 16]);
-      }
-#pragma unroll
-      for (int rr = 1; rr < P; rr++) {
-        int r = p + rr;
-        if (r >= P)
-          r -= P;
-        const cplx *fr = xs_l + (size_t)r * P512_M + u;
-        const cplx *kr = kcol + (size_t)r * P512_M + u;
-#pragma unroll
-        for (int b = 0; b < 16; b++)
-          v[b] = cfma(fr[b * 16], kr[b * 16], v[b]);
-      }
+      n512_mac_ring<P>(v, xs_l, &sm.ring[p * P][0], p, u, SmemLoader());
     } else {
     // the Fourier key of the step streams through a ring of three 8-value chunks
     // (two chunks = 16 x 128-bit loads in flight per thread); the first two are
@@ -283,6 +218,9 @@ pbs_n512_kernel(uint64_t *__restrict__ lwe_out,
     key_chunk(1, kbuf[1]);
     __syncthreads();
     // ---- Fourier MAC: out[b] = sum_r spec_r[b][q] * key[i][p][r][b][q] -------
+    // (restated by the CPU replay, tests/emu/emu_p22.cpp n512_mac_regs: moved
+    // into a shared function, this loop changes the instances' register
+    // allocation)
 #pragma unroll
     for (int ch = 0; ch < 2 * P; ch++) {
       const int r = ch >> 1, hb = (ch & 1) * 8;
@@ -356,15 +294,8 @@ bsk_convert_n512_kernel(cplx *__restrict__ dst, const uint64_t *__restrict__ src
     poly = total_polys - 1;
   const uint32_t c = poly % P, r = (poly / P) % P, i = poly / (P * P);
   const uint64_t *src_p = src + (size_t)poly * P512_N;
-  // 2^-64 / 256 * 2^32 = 2^-40
-  const double scale = 9.094947017729282379150390625e-13;
   cplx v[16];
-#pragma unroll
-  for (int j1 = 0; j1 < 16; j1++) {
-    const uint32_t j = 16u * j1 + u;
-    v[j1] = cmake(ll_to_double((int64_t)src_p[j]) * scale,
-                  ll_to_double((int64_t)src_p[j + P512_M]) * scale);
-  }
+  n512_key_load(src_p, u, v);
   radix16_fwd(v, c_fft256_pass1);
   xq_store_p1(xb[hw], u, v);
   __syncwarp();
