@@ -323,8 +323,9 @@ class CudaRadixServerKey:
     (integer/gpu/server_key/radix/mul.rs:167), and comparisons, selects,
     additions, subtractions, bitwise operations, their clear-operand forms,
     signed overflow flags, abs, erc7984's transfer (`radix`), products and
-    sums (`radix_mul`), divisions (`radix_div`), shifts, rotations and bit counts (`radix_bits`), and vector find
-    and the key-value store's encrypted-key operations (`radix_find`), compiled to KS -> PBS
+    sums (`radix_mul`), divisions (`radix_div`), shifts, rotations and bit counts (`radix_bits`), vector find
+    and the key-value store's encrypted-key operations (`radix_find`), and the oblivious bitonic shuffle
+    of a list of integers by OPRF sort keys (`radix_shuffle`), compiled to KS -> PBS
     layers and run by a bit-circuit runner of its own (created on first use) with `b200_bit_circuit_64_async`.
 
     Those operations take ciphertexts of one kind (unsigned or signed), one
@@ -943,3 +944,32 @@ class CudaRadixServerKey:
         from . import radix_find
 
         return radix_find.kv_store_contains_clear_value(self, store, clear)
+
+    # -- oblivious shuffle (`radix_shuffle`) --------------------------------------
+    def bitonic_shuffle(self, oprf_key, data, key_size, seed):
+        """`data` (single-integer radix ciphertexts of one kind and block count)
+        permuted uniformly at random: sorted by sort keys of `key_size` (a
+        radix_shuffle.BitonicShuffleKeySize) drawn from `seed` by `oprf_key`
+        (an oprf.CudaOprfServerKey) through a bitonic network.  Returns a new
+        list; lists of length 0 or 1 come back as they are."""
+        from . import radix_shuffle
+
+        return radix_shuffle.bitonic_shuffle(self, oprf_key, data, key_size, seed)
+
+    def bitonic_shuffle_and_re_randomize(self, oprf_key, data, key_size, seed, re_randomization_key, prf_context):
+        """`bitonic_shuffle` with the sort keys re-randomized by one list of
+        zeros whose seed derives from `prf_context` (a
+        rerand.ReRandomizationContext, left as it was), the OPRF seed and the
+        keys' bit layout; the same permutation as `bitonic_shuffle`."""
+        from . import radix_shuffle
+
+        return radix_shuffle.bitonic_shuffle_and_re_randomize(self, oprf_key, data, key_size, seed,
+                                                              re_randomization_key, prf_context)
+
+    def bitonic_shuffle_with_keys(self, data, keys):
+        """`data` sorted by `keys` (unsigned radix ciphertexts of one block
+        count, one per element) through the bitonic network; equal keys are
+        ordered as tfhe-rs orders them."""
+        from . import radix_shuffle
+
+        return radix_shuffle.bitonic_shuffle_with_keys(self, data, keys)

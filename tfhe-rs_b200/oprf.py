@@ -289,10 +289,34 @@ class CudaOprfServerKey:
         (shortint generate_oblivious_pseudo_random_bits_chunks): ceil(bc / r)
         blocks, each encrypting a uniform value of r bits, the last one of
         bc % r bits when that is not 0; r = log2(message_modulus)."""
-        from . import gpu
+        flat = self._generate_flat(seed, bit_chunks)
+        return self._chunks(flat.d_vec.t.view(flat.lwe_ciphertext_count, self.big_dim + 1), bit_chunks)
 
+    def generate_oblivious_pseudo_random_bits_chunks_and_re_randomize(self, seed, bit_chunks: Sequence[int],
+                                                                      re_randomization_key, prf_context):
+        """`generate_oblivious_pseudo_random_bits_chunks`, then every block of
+        every chunk re-randomized with one list of zeros drawn from one seed,
+        `rerand.new_prf_rerand_seed(prf_context, seed, RLE of the chunks)`
+        (shortint generate_pseudo_random_bits_chunks_and_re_randomize), on
+        `rerand.re_randomize`.  prf_context: a rerand.ReRandomizationContext,
+        left as it was."""
+        from . import rerand
+        from .integer import CudaUnsignedRadixCiphertext
+
+        if not isinstance(re_randomization_key, rerand.CudaReRandomizationKey):
+            raise ValueError(f"{re_randomization_key!r} is not a CudaReRandomizationKey")
+        rr_seed = rerand.new_prf_rerand_seed(prf_context, seed,
+                                             rle_bytes(bit_chunks, self.message_bits, self.bits_per_block))
         flat = self._generate_flat(seed, bit_chunks)
         t = flat.d_vec.t.view(flat.lwe_ciphertext_count, self.big_dim + 1)
+        if flat.lwe_ciphertext_count:
+            rerand.re_randomize([CudaUnsignedRadixCiphertext(t)], [rr_seed], re_randomization_key, self.streams)
+        return self._chunks(t, bit_chunks)
+
+    def _chunks(self, t, bit_chunks: Sequence[int]):
+        """CudaLweCiphertextList views of the flat blocks `t`, one per chunk"""
+        from . import gpu
+
         chunks, at = [], 0
         for bc in bit_chunks:
             n = -(-int(bc) // self.message_bits)

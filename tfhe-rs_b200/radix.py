@@ -176,10 +176,15 @@ def compare(c: bc.Circuit, lhs: Sequence[Block], rhs: Sequence[Block], op: str, 
 # ---------------------------------------------------------------------------
 # selects
 # ---------------------------------------------------------------------------
-def keep_if(c: bc.Circuit, cond: int, x: Sequence[Block], when: int = 1) -> List[int]:
-    """x where cond == when, else 0: one PBS per block on 4 cond + x"""
-    f = lambda v: (v % MSG_MOD) if v // MSG_MOD == when else 0  # noqa: E731
-    return [_pbs(c, [(cond, MSG_MOD)] + list(b), 0, f) for b in x]
+def keep_if(c: bc.Circuit, cond: int, x: Sequence[Block], when: int = 1, flip: Optional[int] = None) -> List[int]:
+    """x where cond == when, else 0: one PBS per block on 4 cond + x.  With
+    `flip` (an `iconst` bit), x where cond XOR flip == when: the bit enters
+    the same PBS as the body constant 8 flip (value <= 15, no noise)."""
+    if flip is None:
+        f = lambda v: (v % MSG_MOD) if v // MSG_MOD == when else 0  # noqa: E731
+        return [_pbs(c, [(cond, MSG_MOD)] + list(b), 0, f) for b in x]
+    f = lambda v: (v % MSG_MOD) if ((v // MSG_MOD) & 1) ^ (v // (2 * MSG_MOD)) == when else 0  # noqa: E731
+    return [_pbs(c, [(cond, MSG_MOD), (flip, 2 * MSG_MOD)] + list(b), 0, f) for b in x]
 
 
 def if_then_else(c: bc.Circuit, cond: int, a: Sequence[Block], b: Sequence[Block]) -> List[int]:

@@ -94,6 +94,29 @@ class ReRandomizationContext:
     def finalize(self) -> ReRandomizationSeedGen:
         return ReRandomizationSeedGen(self._state.copy(), self._sep)
 
+    def copy(self) -> "ReRandomizationContext":
+        """An independent context with the same hash state (the Rust type's
+        Clone): one context can serve several calls."""
+        out = ReRandomizationContext.__new__(ReRandomizationContext)
+        out._sep, out._state = self._sep, self._state.copy()
+        return out
+
+
+def new_prf_rerand_seed(context: ReRandomizationContext, prf_seed, random_bits_rle: bytes) -> ReRandomizationSeed:
+    """The seed of the zeros that re-randomize one OPRF call's blocks
+    (ReRandomizationSeed::new_prf_rerand_seed, re_randomization.rs): a copy of
+    the context, then the OPRF seed's bytes, then the RLE of the call's random
+    bits (`oprf.rle_bytes`), finalized; its first seed.  `context` is left as
+    it was."""
+    from . import oprf
+
+    if not isinstance(context, ReRandomizationContext):
+        raise ValueError(f"{context!r} is not a ReRandomizationContext")
+    ctx = context.copy()
+    ctx.add_bytes(oprf.seed_bytes(prf_seed))
+    ctx.add_bytes(random_bits_rle)
+    return ctx.finalize().next_seed()
+
 
 def seeds_array(seeds: Sequence[ReRandomizationSeed]) -> np.ndarray:
     """[len(seeds)][40] u8, the layout b200_cpk_encrypt_zeros_from_seeds_64_async reads."""
