@@ -134,6 +134,39 @@ void cuda_programmable_bootstrap_128_async(
 void cleanup_cuda_programmable_bootstrap_128(void *stream, uint32_t gpu_index,
                                              int8_t **pbs_buffer);
 
+/* multi-bit u128 torus (noise squashing with grouped keys),
+ * programmable_bootstrap_multibit.h:18-21, 64-80.  src = HOST standard-domain
+ * key [group][2^g][level][row][col][N] of u128 (GGSW b of a group encrypts the
+ * product of s_u or 1 - s_u as bit g - 1 - u of b is set or clear); dest holds
+ * as many f64 words as src has u64 (layout private).  The PBS reads
+ * num_samples u64 LWEs, LWE lwe_input_indexes[s] (u64) for sample s, and
+ * writes u128 LWEs of k*N + 1 words to rows lwe_output_indexes[s] (u64); one
+ * u128 GLWE LUT of (k+1)*N words serves every sample.  The modulus switch is
+ * the plain one; the degrees are tfhe-rs' modulus_switch_multi_bit.  Shapes:
+ * those of the classic 128-bit PBS, grouping factor 2, 3 or 4, lwe_dimension
+ * a positive multiple of it, num_many_lut = 1; anything else aborts.  One
+ * launch (csrc/pbs128_multibit.cuh, DESIGN.md section 8f); b200_last_pbs_
+ * kernel reports "pbs128_mb<N>". */
+void cuda_convert_lwe_multi_bit_programmable_bootstrap_key_128_async(
+    void *stream, uint32_t gpu_index, void *dest, void const *src,
+    uint32_t input_lwe_dim, uint32_t glwe_dim, uint32_t level_count,
+    uint32_t polynomial_size, uint32_t grouping_factor);
+uint64_t scratch_cuda_multi_bit_programmable_bootstrap_128_async(
+    void *stream, uint32_t gpu_index, int8_t **buffer, uint32_t glwe_dimension,
+    uint32_t polynomial_size, uint32_t level_count,
+    uint32_t input_lwe_ciphertext_count, bool allocate_gpu_memory);
+void cuda_multi_bit_programmable_bootstrap_128_async(
+    void *stream, uint32_t gpu_index, void *lwe_array_out,
+    void const *lwe_output_indexes, void const *lut_vector,
+    void const *lwe_array_in, void const *lwe_input_indexes,
+    void const *bootstrapping_key, int8_t *mem_ptr, uint32_t lwe_dimension,
+    uint32_t glwe_dimension, uint32_t polynomial_size, uint32_t grouping_factor,
+    uint32_t base_log, uint32_t level_count, uint32_t num_samples,
+    uint32_t num_many_lut, uint32_t lut_stride);
+void cleanup_cuda_multi_bit_programmable_bootstrap_128(void *stream,
+                                                       const uint32_t gpu_index,
+                                                       int8_t **buffer);
+
 /* ---- multi-bit PBS: .../include/pbs/programmable_bootstrap_multibit.h:9-42 */
 bool has_support_to_cuda_programmable_bootstrap_cg_multi_bit(
     uint32_t glwe_dimension, uint32_t polynomial_size, uint32_t level_count,
@@ -492,6 +525,20 @@ void b200_apply_noise_squashing_64_async(
     void const *bootstrapping_key, int8_t *buffer, uint32_t lwe_dimension,
     uint32_t glwe_dimension, uint32_t polynomial_size, uint32_t pbs_base_log,
     uint32_t pbs_level_count);
+/* b200_apply_noise_squashing_64_async with a multi-bit squashing key: the
+ * same packing and keyswitch, then cuda_multi_bit_programmable_bootstrap_
+ * 128_async's kernel with grouping_factor and trivial indexes; `buffer` is a
+ * scratch_cuda_multi_bit_programmable_bootstrap_128_async object made for
+ * >= ceil(num_blocks / 2) samples.  Launches, in order: the packing, the
+ * keyswitch, the PBS. */
+void b200_apply_noise_squashing_multi_bit_64_async(
+    void *stream, uint32_t gpu_index, void *lwe_array_out,
+    void const *lwe_array_in, uint32_t num_blocks, uint32_t input_lwe_dimension,
+    uint32_t message_modulus, void const *ksk, uint32_t ks_base_log,
+    uint32_t ks_level_count, void const *lut_vector,
+    void const *bootstrapping_key, int8_t *buffer, uint32_t lwe_dimension,
+    uint32_t glwe_dimension, uint32_t polynomial_size, uint32_t grouping_factor,
+    uint32_t pbs_base_log, uint32_t pbs_level_count);
 /* Noise-squashing compression, the stand-in for cuda_integer_compress_radix_
  * ciphertext_128_async (NoiseSquashingCompressionKey::compress_noise_squashed_
  * ciphertexts_into_list, list_compression/noise_squashing_compression.rs).
@@ -650,7 +697,8 @@ uint64_t b200_kernel_launch_count(void);
  * multi-bit, u32 torus and the PBS of the grouped OPRF), e.g.
  * "n2048_v6<2,true,2,1>", "n512<4,3,true>", "n8192_v2<false>",
  * "multibit_fused<3,2>", "multibit_ll<4,1,tma>", "generic_workspace",
- * "pbs128<2048>" (the 128-bit PBS, by polynomial size); "" before
+ * "pbs128<2048>" (the 128-bit PBS, by polynomial size), "pbs128_mb<2048>"
+ * (the multi-bit 128-bit PBS); "" before
  * the first one.  A static string: valid for the life of the library. */
 const char *b200_last_pbs_kernel(void);
 /* name of the kernel the calling thread's last keyswitch launch ran:

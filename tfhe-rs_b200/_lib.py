@@ -57,6 +57,11 @@ SIGNATURES = {
     "cuda_programmable_bootstrap_128_async": (
         None, [vp, u32, vp, vp, vp, vp, C.POINTER(C.c_int8), u32, u32, u32, u32, u32, u32]),
     "cleanup_cuda_programmable_bootstrap_128": (None, [vp, u32, i8pp]),
+    "cuda_convert_lwe_multi_bit_programmable_bootstrap_key_128_async": (None, [vp, u32, vp, vp, u32, u32, u32, u32, u32]),
+    "scratch_cuda_multi_bit_programmable_bootstrap_128_async": (u64, [vp, u32, i8pp, u32, u32, u32, u32, C.c_bool]),
+    "cuda_multi_bit_programmable_bootstrap_128_async": (
+        None, [vp, u32, vp, vp, vp, vp, vp, vp, C.POINTER(C.c_int8), u32, u32, u32, u32, u32, u32, u32, u32, u32]),
+    "cleanup_cuda_multi_bit_programmable_bootstrap_128": (None, [vp, u32, i8pp]),
     "has_support_to_cuda_programmable_bootstrap_cg_multi_bit": (C.c_bool, [u32, u32, u32, u32, u32]),
     "cuda_convert_lwe_multi_bit_programmable_bootstrap_key_64_async": (None, [vp, u32, vp, vp, u32, u32, u32, u32, u32]),
     "scratch_cuda_multi_bit_programmable_bootstrap_64_async": (u64, [vp, u32, i8pp, u32, u32, u32, u32, C.c_bool]),
@@ -98,6 +103,9 @@ SIGNATURES = {
                u32, u32, u32]),
     "b200_apply_noise_squashing_64_async": (
         None, [vp, u32, vp, vp, u32, u32, u32, vp, u32, u32, vp, vp, C.POINTER(C.c_int8), u32, u32, u32, u32, u32]),
+    "b200_apply_noise_squashing_multi_bit_64_async": (
+        None, [vp, u32, vp, vp, u32, u32, u32, vp, u32, u32, vp, vp, C.POINTER(C.c_int8), u32, u32, u32, u32, u32,
+               u32]),
     "b200_compress_lwe_ciphertexts_128_async": (None, [vp, u32, vp, vp, u32, u32, vp, u32, u32, u32, u32, u32]),
     "b200_decompress_lwe_ciphertexts_128_async": (None, [vp, u32, vp, vp, u32, C.POINTER(u32), u32, u32, u32, u32]),
     "b200_lwe_linear_combination_64_async": (None, [vp, u32, vp, vp, u32, u32, u32, u32, u32, vp, vp, vp, vp]),
@@ -191,10 +199,15 @@ def build(verbose: bool = False) -> str:
 # symbols that only this engine exports (everything else is the reference's ABI)
 ADDITIONS = ("b200_", "cuda_drop_async", "cuda_get_max_shared_memory")
 # reference-ABI symbols outside the 64-bit hot path: a reference build without
-# programmable_bootstrap_classic_128.cu (oracle/build_ref_pbs128.sh adds it) lacks them
+# programmable_bootstrap_classic_128.cu and programmable_bootstrap_multibit_128.cu
+# (oracle/build_ref_pbs128.sh and build_ref_pbs128_mb.sh add them) lacks them
 OPTIONAL_REFERENCE = ("cuda_convert_lwe_programmable_bootstrap_key_128_async",
                       "scratch_cuda_programmable_bootstrap_128_async", "cuda_programmable_bootstrap_128_async",
-                      "cleanup_cuda_programmable_bootstrap_128")
+                      "cleanup_cuda_programmable_bootstrap_128",
+                      "cuda_convert_lwe_multi_bit_programmable_bootstrap_key_128_async",
+                      "scratch_cuda_multi_bit_programmable_bootstrap_128_async",
+                      "cuda_multi_bit_programmable_bootstrap_128_async",
+                      "cleanup_cuda_multi_bit_programmable_bootstrap_128")
 
 
 def load(path: str, strict: bool = True) -> C.CDLL:

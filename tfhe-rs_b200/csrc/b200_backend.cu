@@ -36,6 +36,7 @@
 #include "compression.cuh"
 #include "ciphertext_ops.cuh"
 #include "pbs128.cuh"
+#include "pbs128_multibit.cuh"
 #include "keyswitch128.cuh"
 #include "bit_circuit.cuh"
 #include "msm.cuh"
@@ -1195,6 +1196,68 @@ static void launch_pbs128(cudaStream_t st, uint32_t gpu_index, u128 *lwe_out,
   B200_CHECK(cudaFreeAsync(ws, st));
 }
 
+// ---- multi-bit 128-bit PBS (pbs128_multibit.cuh) ---------------------------------
+// double-double 2N-th roots of unity of the size-2^logM transform (4M entries),
+// created once per device
+static const ddc *dd_roots(uint32_t gpu_index, uint32_t logM) {
+  static std::mutex mutex;
+  static ddc *tables[MAX_GPUS][MAX_LOGM + 1] = {};
+  std::lock_guard<std::mutex> lock(mutex);
+  ddc *&t = tables[gpu_index][logM];
+  if (!t) {
+    std::vector<ddc> host((size_t)4 << logM);
+    b200_fill_dd_roots(logM, host.data());
+    set_device(gpu_index);
+    B200_CHECK(cudaMalloc(&t, host.size() * sizeof(ddc)));
+    B200_CHECK(cudaMemcpy(t, host.data(), host.size() * sizeof(ddc),
+                          cudaMemcpyHostToDevice));
+  }
+  return t;
+}
+
+// the instance for (k, N, l, base_log) and a grouping factor g over n mask
+// words; aborts on an unsupported shape
+static const Pbs128MbInstance &pbs128_mb_instance(uint32_t k, uint32_t N,
+                                                  uint32_t l, uint32_t base_log,
+                                                  uint32_t grouping) {
+  pbs128_instance(k, N, l, base_log); // same (k, N, l) limits as the classic PBS
+  B200_PANIC_IF_FALSE(grouping >= 2 && grouping <= 4,
+                      "Cuda error (multi-bit 128-bit PBS): unsupported "
+                      "grouping factor %u, supported are 2, 3 and 4", grouping);
+  return PBS128_MB_INSTANCES[ilog2_exact(N) - 8];
+}
+static void check_mb_lwe_dimension(uint32_t n, uint32_t grouping) {
+  B200_PANIC_IF_FALSE(n >= grouping && n % grouping == 0,
+                      "Cuda error (multi-bit 128-bit PBS): lwe dimension %u is "
+                      "not a positive multiple of the grouping factor %u", n,
+                      grouping);
+}
+
+static void launch_pbs128_mb(cudaStream_t st, uint32_t gpu_index,
+                             u128 *lwe_out, const uint64_t *out_idx,
+                             const u128 *lut, const uint64_t *lwe_in,
+                             const uint64_t *in_idx, const ddc *bsk,
+                             uint32_t n, uint32_t k, uint32_t N,
+                             uint32_t grouping, uint32_t base_log, uint32_t l,
+                             uint32_t num_samples) {
+  const Pbs128MbInstance &r = pbs128_mb_instance(k, N, l, base_log, grouping);
+  check_mb_lwe_dimension(n, grouping);
+  if (num_samples == 0)
+    return;
+  const uint32_t logM = ilog2_exact(N) - 1;
+  const uint32_t grid = std::min(num_samples, sm_count(gpu_index));
+  const size_t stride = pbs128_ws_bytes(k, N);
+  unsigned char *ws = nullptr;
+  B200_CHECK(cudaMallocFromPoolAsync(&ws, stride * grid,
+                                     workspace_pool(gpu_index), st));
+  launch(r.kernel, {grid, PBS128_THREADS, pbs128_mb_smem_bytes(N), st, gpu_index},
+         lwe_out, out_idx, lut, lwe_in, in_idx, bsk, dd_twiddles(gpu_index, logM),
+         dd_roots(gpu_index, logM), n, k, grouping, base_log, l, num_samples, ws,
+         stride);
+  t_last_pbs_kernel = r.name;
+  B200_CHECK(cudaFreeAsync(ws, st));
+}
+
 // ===========================================================================
 // BLS12-446 multi-scalar multiplication (msm.cuh)
 // ===========================================================================
@@ -1761,6 +1824,79 @@ void cuda_programmable_bootstrap_128_async(
 void cleanup_cuda_programmable_bootstrap_128(void *stream, uint32_t gpu_index,
                                              int8_t **pbs_buffer) {
   cleanup_cuda_programmable_bootstrap_64(stream, gpu_index, pbs_buffer);
+}
+
+// ---- multi-bit u128 torus (programmable_bootstrap_multibit.h:18-21,64-80) ----
+void cuda_convert_lwe_multi_bit_programmable_bootstrap_key_128_async(
+    void *stream, uint32_t gpu_index, void *dest, void const *src,
+    uint32_t input_lwe_dim, uint32_t glwe_dim, uint32_t level_count,
+    uint32_t polynomial_size, uint32_t grouping_factor) {
+  set_device(gpu_index);
+  const uint32_t k = glwe_dim, N = polynomial_size, l = level_count;
+  pbs128_mb_instance(k, N, l, 1, grouping_factor);
+  check_mb_lwe_dimension(input_lwe_dim, grouping_factor);
+  // [group][2^g][l][k+1][k+1] polynomials: the classic conversion over more
+  const PbsParams p{input_lwe_dim, k, N, 1, l, grouping_factor};
+  const size_t polys = (size_t)p.num_ggsw() * l * (k + 1) * (k + 1);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  u128 *staging = nullptr;
+  B200_CHECK(cudaMallocAsync(&staging, polys * N * sizeof(u128), st));
+  B200_CHECK(cudaMemcpyAsync(staging, src, polys * N * sizeof(u128),
+                             cudaMemcpyHostToDevice, st));
+  launch(pbs128_instance(k, N, l, 1).convert,
+         {(unsigned)polys, 256, (N / 2) * sizeof(ddc), st, gpu_index},
+         static_cast<ddc *>(dest), staging,
+         dd_twiddles(gpu_index, ilog2_exact(N) - 1));
+  B200_CHECK(cudaFreeAsync(staging, st));
+}
+
+uint64_t scratch_cuda_multi_bit_programmable_bootstrap_128_async(
+    void *stream, uint32_t gpu_index, int8_t **buffer, uint32_t glwe_dimension,
+    uint32_t polynomial_size, uint32_t level_count,
+    uint32_t input_lwe_ciphertext_count, bool allocate_gpu_memory) {
+  (void)stream;
+  set_device(gpu_index);
+  pbs128_instance(glwe_dimension, polynomial_size, level_count, 1);
+  // both tables are built here (set-up call), so that the bootstrap itself
+  // never runs a synchronous copy
+  dd_twiddles(gpu_index, ilog2_exact(polynomial_size) - 1);
+  dd_roots(gpu_index, ilog2_exact(polynomial_size) - 1);
+  return new_pbs_scratch(buffer, MULTI_BIT, glwe_dimension, polynomial_size,
+                         level_count, input_lwe_ciphertext_count,
+                         allocate_gpu_memory, 0, true);
+}
+
+void cuda_multi_bit_programmable_bootstrap_128_async(
+    void *stream, uint32_t gpu_index, void *lwe_array_out,
+    void const *lwe_output_indexes, void const *lut_vector,
+    void const *lwe_array_in, void const *lwe_input_indexes,
+    void const *bootstrapping_key, int8_t *mem_ptr, uint32_t lwe_dimension,
+    uint32_t glwe_dimension, uint32_t polynomial_size, uint32_t grouping_factor,
+    uint32_t base_log, uint32_t level_count, uint32_t num_samples,
+    uint32_t num_many_lut, uint32_t lut_stride) {
+  (void)lut_stride;
+  set_device(gpu_index);
+  B200_PANIC_IF_FALSE(num_many_lut == 1, "Cuda error (multi-bit 128-bit PBS): "
+                      "num_many_lut must be 1, got %u", num_many_lut);
+  pbs_scratch(mem_ptr, MULTI_BIT, "multi-bit 128-bit PBS",
+              PbsParams{lwe_dimension, glwe_dimension, polynomial_size,
+                        base_log, level_count, grouping_factor},
+              num_samples, true);
+  launch_pbs128_mb(static_cast<cudaStream_t>(stream), gpu_index,
+                   static_cast<u128 *>(lwe_array_out),
+                   static_cast<const uint64_t *>(lwe_output_indexes),
+                   static_cast<const u128 *>(lut_vector),
+                   static_cast<const uint64_t *>(lwe_array_in),
+                   static_cast<const uint64_t *>(lwe_input_indexes),
+                   static_cast<const ddc *>(bootstrapping_key), lwe_dimension,
+                   glwe_dimension, polynomial_size, grouping_factor, base_log,
+                   level_count, num_samples);
+}
+
+void cleanup_cuda_multi_bit_programmable_bootstrap_128(void *stream,
+                                                       const uint32_t gpu_index,
+                                                       int8_t **buffer) {
+  cleanup_cuda_programmable_bootstrap_64(stream, gpu_index, buffer);
 }
 
 // ===========================================================================
@@ -2520,6 +2656,46 @@ void b200_apply_noise_squashing_64_async(
                 static_cast<const ddc *>(bootstrapping_key), lwe_dimension,
                 glwe_dimension, polynomial_size, pbs_base_log, pbs_level_count,
                 packed, s.centered_ms);
+  B200_CHECK(cudaFreeAsync(ws, st));
+}
+
+void b200_apply_noise_squashing_multi_bit_64_async(
+    void *stream, uint32_t gpu_index, void *lwe_array_out,
+    void const *lwe_array_in, uint32_t num_blocks, uint32_t input_lwe_dimension,
+    uint32_t message_modulus, void const *ksk, uint32_t ks_base_log,
+    uint32_t ks_level_count, void const *lut_vector,
+    void const *bootstrapping_key, int8_t *buffer, uint32_t lwe_dimension,
+    uint32_t glwe_dimension, uint32_t polynomial_size, uint32_t grouping_factor,
+    uint32_t pbs_base_log, uint32_t pbs_level_count) {
+  set_device(gpu_index);
+  pbs128_mb_instance(glwe_dimension, polynomial_size, pbs_level_count,
+                     pbs_base_log, grouping_factor);
+  check_mb_lwe_dimension(lwe_dimension, grouping_factor);
+  const uint32_t packed = (num_blocks + 1) / 2;
+  const PbsParams p{lwe_dimension, glwe_dimension, polynomial_size,
+                    pbs_base_log, pbs_level_count, grouping_factor};
+  pbs_scratch(buffer, p.type(), "multi-bit noise squashing", p, packed, true);
+  if (num_blocks == 0)
+    return;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const uint64_t big_words = (uint64_t)packed * (input_lwe_dimension + 1);
+  const uint64_t small_words = (uint64_t)packed * (lwe_dimension + 1);
+  uint64_t *ws = nullptr;
+  B200_CHECK(cudaMallocFromPoolAsync(&ws, (big_words + small_words) * sizeof(uint64_t),
+                                     workspace_pool(gpu_index), st));
+  uint64_t *pairs = ws, *small = ws + big_words;
+  launch(squash_pack_pairs_kernel,
+         {(unsigned)((big_words + 255) / 256), 256, 0, st, gpu_index}, pairs,
+         static_cast<const uint64_t *>(lwe_array_in), input_lwe_dimension + 1,
+         num_blocks, (uint64_t)message_modulus);
+  keyswitch_64(stream, gpu_index, small, nullptr, pairs, nullptr, ksk,
+               input_lwe_dimension, lwe_dimension + 1, lwe_dimension,
+               ks_base_log, ks_level_count, packed);
+  launch_pbs128_mb(st, gpu_index, static_cast<u128 *>(lwe_array_out), nullptr,
+                   static_cast<const u128 *>(lut_vector), small, nullptr,
+                   static_cast<const ddc *>(bootstrapping_key), lwe_dimension,
+                   glwe_dimension, polynomial_size, grouping_factor,
+                   pbs_base_log, pbs_level_count, packed);
   B200_CHECK(cudaFreeAsync(ws, st));
 }
 

@@ -137,3 +137,75 @@ B200_HD void p128_load_key_poly(const u128 *p, ddc *buf, uint32_t M,
     buf[j] = ddc_make(dd_scale(i128_to_dd(p[j]), inv_m),
                       dd_scale(i128_to_dd(p[j + M]), inv_m));
 }
+
+// ---- multi-bit (pbs128_multibit.cuh) ----------------------------------------
+// the 2N-th roots of unity in double-double, root[e] = exp(i pi e / N) for
+// e < 2N = 4M (host): slot pos of X^d is root[d (1 + 4 bitrev(pos)) mod 2N]
+static inline void b200_fill_dd_roots(uint32_t logM, ddc *root) {
+  const uint64_t cnt = (uint64_t)4 << logM;
+  for (uint64_t e = 0; e < cnt; e++)
+    root[e] = dd_unit_root(e, cnt);
+}
+
+// monomial degree of GGSW `b` of a group of g mask words
+// (modulus_switch_multi_bit): the selected u64 words are summed, then switched
+// once; mask word u is selected by bit g - 1 - u of b (selection_bit)
+B200_HD uint32_t p128_mb_degree(const uint64_t *mask, uint32_t g, uint32_t b,
+                                uint32_t log_mod) {
+  uint64_t sum = 0;
+  for (uint32_t u = 0; u < g; u++)
+    if ((b >> (g - 1 - u)) & 1u)
+      sum += mask[u];
+  return modulus_switch_u64(sum, log_mod);
+}
+
+// digit polynomial t of acc_r itself into buf (the multi-bit step decomposes
+// the accumulator, not acc * X^a - acc)
+B200_HD void p128_decompose_acc(const u128 *acc_r, ddc *buf, uint32_t N,
+                                uint32_t base_log, uint32_t l, uint32_t t,
+                                uint32_t tid, uint32_t nthreads) {
+  const uint32_t M = N >> 1;
+  for (uint32_t j = tid; j < M; j += nthreads) {
+    u128 s0 = decomp128_init_state(acc_r[j], base_log, l);
+    u128 s1 = decomp128_init_state(acc_r[j + M], base_log, l);
+    i128 d0 = 0, d1 = 0;
+    for (uint32_t u = 0; u <= t; u++) {
+      d0 = decomp128_next_digit(&s0, base_log);
+      d1 = decomp128_next_digit(&s1, base_log);
+    }
+    buf[j] = ddc_make(i128_to_dd((u128)d0), i128_to_dd((u128)d1));
+  }
+}
+
+// out[c][pos] (+)= buf[pos] * sum_b X^{deg_b} G_b[c][pos], c = 0..k: the
+// multi-bit bundle folded into the MAC slot by slot.  `g` points at the
+// [k+1][M] key spectra of one (level, row) of GGSW 0 of the group; GGSW b is
+// `ggsw_len` ddc further per b.  degs[b] for b = 1..nggsw-1.
+B200_HD void p128_mb_mac(const ddc *buf, ddc *out, const ddc *g,
+                         size_t ggsw_len, uint32_t nggsw, const uint32_t *degs,
+                         const ddc *root, uint32_t logM, uint32_t k,
+                         bool first, uint32_t tid, uint32_t nthreads) {
+  const uint32_t M = 1u << logM, emask = (4u << logM) - 1;
+  for (uint32_t pos = tid; pos < M; pos += nthreads) {
+    const ddc f = buf[pos];
+    const uint32_t kf = 1u + 4u * gen_bitrev(pos, logM);
+    for (uint32_t c = 0; c <= k; c++) {
+      const size_t off = (size_t)c * M + pos;
+      ddc gv = g[off];
+      for (uint32_t b = 1; b < nggsw; b++)
+        gv = ddc_fma(g[b * ggsw_len + off], root[(degs[b] * kf) & emask], gv);
+      ddc *o = out + off;
+      *o = first ? ddc_mul(f, gv) : ddc_fma(f, gv, *o);
+    }
+  }
+}
+
+// acc_c = round(buf) modulo 2^128
+B200_HD void p128_acc_assign(u128 *acc_c, const ddc *buf, uint32_t M,
+                             uint32_t tid, uint32_t nthreads) {
+  for (uint32_t j = tid; j < M; j += nthreads) {
+    const ddc v = buf[j];
+    acc_c[j] = dd_to_u128(v.re);
+    acc_c[j + M] = dd_to_u128(v.im);
+  }
+}
